@@ -12,7 +12,8 @@
  *   - Every function returns an idb_status; idb_last_error() gives the thread-local message.
  *   - There is NO CPU fallback: without a CUDA device every compute call returns IDB_ERR_CUDA.
  *   - Points are f32 vectors under squared-L2 (the reference's FloatArray metric, py:378-421), any dim >= 1,
- *     computed in one canonical fp32 summation order (DESIGN.md) so results are bit-reproducible.
+ *     computed in one canonical fp32 summation order (DESIGN.md) so results are bit-reproducible.  The entry points without an
+ *     `_ex` suffix are squared-L2 indexes; the `_ex` ones also take IDB_METRIC_COSINE (DESIGN.md §3a).
  *   - PointIds are u32; IDB_INVALID (u32::MAX) is the reference's INVALID sentinel (types:293).
  */
 #ifndef INSTANT_DISTANCE_B200_H
@@ -28,6 +29,13 @@ extern "C" {
 #define IDB_INVALID 0xFFFFFFFFu
 #define IDB_STORAGE_F32 0u
 #define IDB_STORAGE_BF16 1u
+/* Metrics (DESIGN.md §3a).  IDB_METRIC_COSINE: every row and every query is normalised in the canonical order (x / sqrt(sum x^2),
+ * correctly rounded; a row whose sum of squares overflows becomes zeros and NaN), the traversal runs the canonical squared L2 on
+ * the normalised rows, and the reported distance is half of it: 1 - cos(x, y) (0 .. 2).  An all-zero row stays zero, so it is at
+ * 0.5 from every other row and at 0 from another zero row.  An index stores the normalised rows (bf16: normalised in f32, then
+ * rounded) and exports / saves them. */
+#define IDB_METRIC_L2SQ 0u
+#define IDB_METRIC_COSINE 1u
 
 #if defined(__GNUC__)
 #define IDB_API __attribute__((visibility("default")))
@@ -80,6 +88,11 @@ IDB_API idb_status idb_params_default(idb_params* p);
  * rows: n x dim row-major host f32.  out_ids[i] = PointId assigned to input row i (core:262-270); may be NULL. */
 IDB_API idb_status idb_build_f32(const float* rows, uint64_t n, uint32_t dim, const idb_params* params,
                          idb_index** out_index, uint32_t* out_ids);
+/* Same, for an index of metric `metric` (IDB_METRIC_*); idb_build_f32 = IDB_METRIC_L2SQ.  With IDB_METRIC_COSINE the rows are
+ * normalised before the build (the caller's rows are not written).  (The metric is an argument rather than an idb_params field so
+ * that idb_params keeps its size: callers compiled against an earlier header allocate it themselves.) */
+IDB_API idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, const idb_params* params, uint32_t metric,
+                                idb_index** out_index, uint32_t* out_ids);
 
 /* "Search a given graph": adopt a graph built elsewhere (the reference, the oracle, a loaded .idx file).
  * This is the parity entry point.  Mirrors the fields of `Hnsw` (core:194-199):
@@ -95,6 +108,19 @@ IDB_API idb_status idb_index_from_graph_f32(const float* points, uint64_t n, uin
 IDB_API idb_status idb_index_from_graph_bf16(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
                                      const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
                                      const uint64_t* upper_n, int32_t device, idb_index** out_index);
+
+/* Both of the above and the metric: storage = IDB_STORAGE_*, metric = IDB_METRIC_*.  With IDB_METRIC_COSINE the points are taken
+ * as given (normalising is not idempotent bit for bit, so an adopted graph keeps the exact rows it was built on): every row must
+ * be all zeros or have |sum x^2 - 1| <= 1e-2 (which lets bf16-rounded unit rows through), else IDB_ERR_INVALID_ARG.
+ * idb_normalize_f32 gives the canonical normalisation. */
+IDB_API idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
+                                           const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
+                                           const uint64_t* upper_n, uint32_t storage, uint32_t metric, int32_t device,
+                                           idb_index** out_index);
+
+/* The canonical normalisation of n rows of dim f32 (DESIGN.md §3a) on the device: out (n x dim, host) = what a cosine index
+ * stores for `rows` (before any bf16 rounding).  For callers preparing rows for idb_index_from_graph_ex, and for parity tests. */
+IDB_API idb_status idb_normalize_f32(const float* rows, uint64_t n, uint32_t dim, int32_t device, float* out);
 
 /* Hnsw::search(point, &mut Search) (core:352-383), batched: one independent search per query row.
  * The reference returns the whole `nearest` list (<= ef_search items, ascending by (distance, pid));
@@ -152,6 +178,8 @@ typedef struct idb_info {
     uint32_t storage;           /* IDB_STORAGE_* */
 } idb_info;
 IDB_API idb_status idb_index_info(const idb_index* index, idb_info* out);
+/* The index's IDB_METRIC_* (a separate call, so that idb_info keeps its size). */
+IDB_API idb_status idb_index_metric(const idb_index* index, uint32_t* out_metric);
 IDB_API idb_status idb_index_export_points(const idb_index* index, float* out /* n x dim */);
 IDB_API idb_status idb_index_export_zero(const idb_index* index, uint32_t* out /* n x 2M */);
 IDB_API idb_status idb_index_export_upper(const idb_index* index, uint32_t layer /* 1-based */, uint32_t* out /* n_l x M */);
@@ -161,6 +189,11 @@ IDB_API idb_status idb_index_export_upper(const idb_index* index, uint32_t layer
  * them.  *out_values_offset (may be NULL) = file offset where an HnswMap's `values` begin (core:131-134), or the file size. */
 IDB_API idb_status idb_index_save(const idb_index* index, const char* path);
 IDB_API idb_status idb_index_load(const char* path, uint32_t dim, uint32_t M, int32_t device, idb_index** out_index, uint64_t* out_values_offset);
+/* Same, as an index of metric `metric`; idb_index_load = IDB_METRIC_L2SQ.  The file format does not change and does not record the
+ * metric: a cosine index saves its normalised rows, and loading them as cosine takes them as given (rows that are neither unit
+ * length nor all zeros: IDB_ERR_FORMAT). */
+IDB_API idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M, uint32_t metric, int32_t device, idb_index** out_index,
+                                     uint64_t* out_values_offset);
 
 /* Measurement hooks (bench.py): when enabled, CUDA events are recorded on the index stream immediately around the
  * dominant kernel of each call (K1 search_layer for searches); idb_index_last_kernel_ms waits for that kernel and
@@ -187,7 +220,9 @@ IDB_API void idb_index_free(idb_index* index);         /* Drop for Hnsw */
  * The reference has no distributed path; this is north_star's layout: every rank owns an independent index over its
  * contiguous range of the input rows, every query is searched on every shard, and ONE ncclAllGather of the per-shard
  * top-k (packed (distance, global id) keys) is followed by a merge kernel.  Results: the k smallest (distance, global id)
- * of the union of the shards' `nearest` lists; identical on every rank. */
+ * of the union of the shards' `nearest` lists; identical on every rank.
+ * Metric: the shards of one call must share one metric (else IDB_ERR_INVALID_ARG).  Across ranks that cannot be checked without
+ * another collective, so it is the caller's contract: every rank's shards must have the same metric. */
 #define IDB_UNIQUE_ID_BYTES 128
 typedef struct idb_comm idb_comm;
 IDB_API idb_status idb_comm_unique_id(void* out_unique_id /* IDB_UNIQUE_ID_BYTES, made on one rank, shared by the host app */);

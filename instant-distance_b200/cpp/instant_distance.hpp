@@ -158,6 +158,7 @@ class Builder {
     uint64_t seed_ = 0;
     uint32_t m_ = 32;
     int device_ = 0;
+    uint32_t metric_ = IDB_METRIC_L2SQ;
 
   public:
     Builder() {
@@ -171,6 +172,9 @@ class Builder {
     Builder& ml(float v) { ml_ = v; return *this; }
     Builder& seed(uint64_t v) { seed_ = v; return *this; }
     Builder& device(int d) { device_ = d; return *this; }  // not in the reference: which GPU
+    // Not in the reference: IDB_METRIC_L2SQ (default) or IDB_METRIC_COSINE — searches then report 1 - cos (DESIGN.md §3a);
+    // Point::distance stays squared L2.
+    Builder& metric(uint32_t m) { metric_ = m; return *this; }
     std::tuple<size_t, size_t, float, uint64_t> into_parts() const { return {ef_search_, ef_construction_, ml_, seed_}; }
 
     // Builder::build_hnsw (lib.rs:83-85)
@@ -195,7 +199,7 @@ class Builder {
         p.device = device_;
         std::vector<uint32_t> ids(points.size());
         Hnsw h;
-        check(idb_build_f32(flat.data(), points.size(), dim, &p, &h.raw_, ids.data()));
+        check(idb_build_ex(flat.data(), points.size(), dim, &p, metric_, &h.raw_, ids.data()));
         h.ef_search_ = ef_search_;
         h.points_.resize(points.size());
         std::vector<PointId> out(points.size());

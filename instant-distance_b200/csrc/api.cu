@@ -62,6 +62,22 @@ __global__ void distance_kernel(const float4* a, const float4* b, uint32_t nchun
     if (lane == 0) *out = s;
 }
 
+// One warp per row: the canonical normalisation (hnsw_device.cuh normalize_row).  No __restrict__ / __ldg: dst may alias src.
+__global__ void normalize_rows_kernel(const float* src, uint64_t src_stride, float4* dst, uint64_t n, uint32_t dim, uint32_t nchunks) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t wpb = blockDim.x >> 5;
+    for (uint64_t r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += (uint64_t)gridDim.x * wpb)
+        normalize_row(src + r * src_stride, dim, dst + r * nchunks, nchunks, lane);
+}
+
+cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,
+                           cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint64_t blocks = std::min<uint64_t>((n + 7) / 8, (uint64_t)num_sms * 16);
+    normalize_rows_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, src_stride, reinterpret_cast<float4*>(dst), n, dim, nchunks);
+    return cudaGetLastError();
+}
+
 // f32 -> bf16 (round to nearest even) and back (exact), element-wise over the padded row matrix
 __global__ void narrow_bf16_kernel(const float* src, uint16_t* dst, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -343,7 +359,7 @@ void HostOut::finish() const {
 
 void Lane::free_all() {
     cudaFree(ctrl); cudaFree(status); cudaFree(fail_list); cudaFree(counters);
-    cudaFree(q); cudaFree(ids); cudaFree(dist); cudaFree(len);
+    cudaFree(q); cudaFree(qn); cudaFree(ids); cudaFree(dist); cudaFree(len);
     cudaFree(keys_local); cudaFree(keys_all); cudaFree(q2); cudaFree(ids2);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
@@ -483,9 +499,8 @@ idb_status Index::select_visited_tier(uint32_t ef, SearchArgs& a, LaunchWindow& 
 
 int Index::search_grid() const { return num_sms * ctx->slots_per_sm; }
 
-// Enqueue one batched search on a lane; all pointers are device pointers, d_queries padded to nchunks*4 floats per row.
-// The caller holds ln.mu.
-idb_status Index::enqueue_search(Lane& ln, const float* d_queries_padded, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
+// Enqueue one batched search on a lane; all pointers are device pointers (d_queries: see internal.cuh).  The caller holds ln.mu.
+idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
                                  float* d_dist, uint32_t* d_len, uint64_t* out_keys) {
     if (n) ef = (uint32_t)std::min<uint64_t>(ef, n);  // admission is rank < ef and there are only n distinct ids: same results
     if (ef > 1024) return fail(IDB_ERR_UNSUPPORTED, "ef_search %u > 1024 (on an index of more than 1024 points) is not supported", ef);
@@ -496,7 +511,8 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries_padded, uint64
     SearchArgs a;
     std::memset(&a, 0, sizeof(a));
     a.g = view();
-    a.queries = reinterpret_cast<const float4*>(d_queries_padded);
+    a.queries = reinterpret_cast<const float4*>(d_queries);
+    a.metric = metric;
     a.n_work = nq;
     a.ef = ef;
     a.k = k;
@@ -518,6 +534,11 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries_padded, uint64
     const int row_t = (int)((2 * M + 31) / 32);
     const int ef_t = (int)((ef + 31) / 32);
     const int grid = std::max(1, (int)std::min<uint64_t>((nq + kSearchWarps - 1) / kSearchWarps, (uint64_t)search_grid()));
+    if (metric == kMetricCosine) {  // once per call: K1 and the retry pass read the same normalised rows; the caller's stay untouched
+        CUDA_TRY(ensure(ln.qn, ln.qn_cap, nq * nchunks * 4));
+        CUDA_TRY(normalize_rows(d_queries, q_stride, ln.qn, nq, dim, nchunks, num_sms, ln.stream));
+        a.queries = reinterpret_cast<const float4*>(ln.qn);
+    }
 
     std::lock_guard<std::mutex> lk(ctx->mu);  // the tables this launch uses must not be regrown under it
     LaunchWindow win;
@@ -527,7 +548,7 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries_padded, uint64
     if (profiling) CUDA_TRY(cudaEventRecord(ln.ev0, ln.stream));
     CUDA_TRY(dispatch_search(a, ch, row_t, ef_t, grid, ln.stream, win));
     if (profiling) CUDA_TRY(cudaEventRecord(ln.ev1, ln.stream));
-    ln.last_launches = 2;  // K1 + the (normally idle) retry pass
+    ln.last_launches = metric == kMetricCosine ? 3 : 2;  // (the query normalisation) + K1 + the (normally idle) retry pass
 
     // Retry pass (device-side, unconditional, normally a no-op): queries whose visited table overflowed are re-run
     // by a few warps with 2^18-slot hash sets.  n_work is read from fail_count on the device.
@@ -751,9 +772,9 @@ idb_status idb_params_default(idb_params* p) {
     return IDB_OK;
 }
 
-static idb_status index_from_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
-                                   const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
-                                   const uint64_t* upper_n, int32_t device, bool bf16, idb_index** out_index) {
+idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search, const uint32_t* zero,
+                                   uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n, uint32_t storage,
+                                   uint32_t metric, int32_t device, idb_index** out_index) {
     if (!out_index) return fail(IDB_ERR_INVALID_ARG, "out_index is null");
     *out_index = nullptr;
     if (dim == 0) return fail(IDB_ERR_INVALID_ARG, "dim must be >= 1");
@@ -762,11 +783,30 @@ static idb_status index_from_graph(const float* points, uint64_t n, uint32_t dim
     if (n && (!points || !zero)) return fail(IDB_ERR_INVALID_ARG, "points/zero is null");
     if (n_upper > 31) return fail(IDB_ERR_INVALID_ARG, "too many layers");
     if (n_upper && (!upper || !upper_n)) return fail(IDB_ERR_INVALID_ARG, "upper/upper_n is null");
+    if (storage != IDB_STORAGE_F32 && storage != IDB_STORAGE_BF16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
+    if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
+    if (metric == IDB_METRIC_COSINE) {
+        // Adopted rows are stored as given (normalising is not idempotent bit for bit), so they must already be unit rows; the
+        // tolerance lets bf16-rounded unit rows through.
+        for (uint64_t r = 0; r < n; ++r) {
+            const float* x = points + r * dim;
+            double s = 0.0;
+            bool all_zero = true;
+            for (uint32_t i = 0; i < dim; ++i) {
+                s += (double)x[i] * x[i];
+                all_zero = all_zero && x[i] == 0.f;
+            }
+            if (!all_zero && !(std::fabs(s - 1.0) <= 1e-2))
+                return fail(IDB_ERR_INVALID_ARG, "cosine index: row %llu has squared norm %g; rows must be unit length or all zeros "
+                            "(idb_normalize_f32 gives the canonical normalisation)", (unsigned long long)r, s);
+        }
+    }
     auto* ix = new (std::nothrow) Index();
     if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
+    ix->metric = metric;
     idb_status st = ix->init_device(device);
     if (st == IDB_OK) st = ix->upload(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n);
-    if (st == IDB_OK && bf16) st = ix->narrow_points_to_bf16();
+    if (st == IDB_OK && storage == IDB_STORAGE_BF16) st = ix->narrow_points_to_bf16();
     if (st != IDB_OK) { delete ix; return st; }
     *out_index = reinterpret_cast<idb_index*>(ix);
     return IDB_OK;
@@ -775,13 +815,15 @@ static idb_status index_from_graph(const float* points, uint64_t n, uint32_t dim
 idb_status idb_index_from_graph_f32(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
                                     const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
                                     const uint64_t* upper_n, int32_t device, idb_index** out_index) {
-    return index_from_graph(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n, device, false, out_index);
+    return idb_index_from_graph_ex(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n, IDB_STORAGE_F32, IDB_METRIC_L2SQ, device,
+                                   out_index);
 }
 
 idb_status idb_index_from_graph_bf16(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
                                      const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
                                      const uint64_t* upper_n, int32_t device, idb_index** out_index) {
-    return index_from_graph(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n, device, true, out_index);
+    return idb_index_from_graph_ex(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n, IDB_STORAGE_BF16, IDB_METRIC_L2SQ, device,
+                                   out_index);
 }
 
 }  // extern "C"
@@ -799,6 +841,8 @@ static idb_status search_device_on_lane(Index* ix, Lane& ln, const float* d_quer
         ln.last_nq = 0;
         return IDB_OK;
     }
+    if (ix->metric == kMetricCosine)  // the normalisation writes padded rows itself
+        return ix->enqueue_search(ln, d_queries, ix->dim, nq, ef, k, d_out_ids, d_out_dist, d_out_len, out_keys);
     const float* qp = d_queries;
     const size_t stride = (size_t)ix->nchunks * 4;
     if (stride != ix->dim || (reinterpret_cast<uintptr_t>(d_queries) & 15)) {
@@ -807,7 +851,7 @@ static idb_status search_device_on_lane(Index* ix, Lane& ln, const float* d_quer
         CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, d_queries, ix->dim * 4, ix->dim * 4, nq, cudaMemcpyDeviceToDevice, ln.stream));
         qp = ln.q;
     }
-    return ix->enqueue_search(ln, qp, nq, ef, k, d_out_ids, d_out_dist, d_out_len, out_keys);
+    return ix->enqueue_search(ln, qp, stride, nq, ef, k, d_out_ids, d_out_dist, d_out_len, out_keys);
 }
 
 // used by sharded.cu: lane 0, caller holds its mutex
@@ -863,13 +907,15 @@ idb_status idb_search_batch_f32(idb_index* index, const float* queries, uint64_t
     CUDA_TRY(ensure(ln.ids, ln.ids_cap, nq * k));
     CUDA_TRY(ensure(ln.dist, ln.dist_cap, nq * k));
     CUDA_TRY(ensure(ln.len, ln.len_cap, nq));
-    if (stride == ix->dim) {
-        CUDA_TRY(cudaMemcpyAsync(ln.q, queries, nq * stride * 4, cudaMemcpyHostToDevice, ln.stream));
+    uint64_t q_stride = stride;
+    if (stride == ix->dim || ix->metric == kMetricCosine) {  // (cosine: the normalisation writes padded rows itself)
+        CUDA_TRY(cudaMemcpyAsync(ln.q, queries, nq * ix->dim * 4, cudaMemcpyHostToDevice, ln.stream));
+        q_stride = ix->dim;
     } else {
         CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, ln.stream));
         CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, queries, ix->dim * 4, ix->dim * 4, nq, cudaMemcpyHostToDevice, ln.stream));
     }
-    idb_status st = ix->enqueue_search(ln, ln.q, nq, ef, k, ln.ids, ln.dist, ln.len, nullptr);
+    idb_status st = ix->enqueue_search(ln, ln.q, q_stride, nq, ef, k, ln.ids, ln.dist, ln.len, nullptr);
     if (st != IDB_OK) return st;
     HostOut ho;
     ho.add(out_ids, ln.ids, nq * k * 4);
@@ -1057,6 +1103,35 @@ idb_status idb_distance_f32(const float* a, const float* b, uint32_t dim, int32_
     cudaError_t e = cudaMemcpy(out, d + 2 * (size_t)nchunks * 4, 4, cudaMemcpyDeviceToHost);
     cudaFree(d);
     if (e != cudaSuccess) return fail(IDB_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
+    return IDB_OK;
+}
+
+idb_status idb_normalize_f32(const float* rows, uint64_t n, uint32_t dim, int32_t device, float* out) {
+    if (dim == 0 || (n && (!rows || !out))) return fail(IDB_ERR_INVALID_ARG, "null argument or dim == 0");
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
+        return fail(IDB_ERR_CUDA, "no CUDA device available; this library has no CPU fallback");
+    if (device < 0 || device >= count) return fail(IDB_ERR_INVALID_ARG, "device %d out of range (0..%d)", device, count - 1);
+    if (n == 0) return IDB_OK;
+    CUDA_TRY(cudaSetDevice(device));
+    int num_sms = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, device));
+    const uint32_t nchunks = (dim + 3) / 4;
+    const size_t in_floats = n * (size_t)dim, in_padded = (in_floats + 3) / 4 * 4, out_floats = n * (size_t)nchunks * 4;
+    float* d = nullptr;
+    CUDA_TRY(cudaMalloc(&d, (in_padded + out_floats) * sizeof(float)));
+    float* d_out = d + in_padded;  // 16-byte aligned
+    cudaError_t e = cudaMemcpy(d, rows, in_floats * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = normalize_rows(d, dim, d_out, n, dim, nchunks, num_sms, 0);
+    if (e == cudaSuccess) e = cudaMemcpy2D(out, dim * sizeof(float), d_out, nchunks * 4 * sizeof(float), dim * sizeof(float), n, cudaMemcpyDeviceToHost);
+    cudaFree(d);
+    if (e != cudaSuccess) return fail(IDB_ERR_CUDA, "CUDA error: %s", cudaGetErrorString(e));
+    return IDB_OK;
+}
+
+idb_status idb_index_metric(const idb_index* index, uint32_t* out) {
+    if (!index || !out) return fail(IDB_ERR_INVALID_ARG, "null argument");
+    *out = reinterpret_cast<const Index*>(index)->metric;
     return IDB_OK;
 }
 

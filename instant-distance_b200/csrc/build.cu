@@ -196,6 +196,8 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
         CUDA_TRY(cudaMemcpyAsync(d_order, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
         gather_rows_kernel<<<ix->num_sms * 8, 256, 0, st>>>(d_rows, d_order, ix->d_points, n, dim, (uint32_t)stride);
         CUDA_TRY(cudaGetLastError());
+        if (ix->metric == kMetricCosine)  // DESIGN §3a: a cosine index stores the normalised rows (bf16: normalised, then rounded)
+            CUDA_TRY(normalize_rows(ix->d_points, stride, ix->d_points, n, dim, ix->nchunks, ix->num_sms, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         cudaFree(d_rows);
         cudaFree(d_order);
@@ -371,7 +373,13 @@ using namespace idb;
 
 extern "C" idb_status idb_build_f32(const float* rows, uint64_t n, uint32_t dim, const idb_params* params, idb_index** out_index,
                                     uint32_t* out_ids) {
+    return idb_build_ex(rows, n, dim, params, IDB_METRIC_L2SQ, out_index, out_ids);
+}
+
+extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, const idb_params* params, uint32_t metric,
+                                   idb_index** out_index, uint32_t* out_ids) {
     if (!out_index) return fail(IDB_ERR_INVALID_ARG, "out_index is null");
+    if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
     *out_index = nullptr;
     if (!params) return fail(IDB_ERR_INVALID_ARG, "params is null");
     if (dim == 0) return fail(IDB_ERR_INVALID_ARG, "dim must be >= 1");
@@ -389,6 +397,7 @@ extern "C" idb_status idb_build_f32(const float* rows, uint64_t n, uint32_t dim,
                     "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns");
     auto* ix = new (std::nothrow) Index();
     if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
+    ix->metric = metric;
     idb_status st = ix->init_device(params->device);
     if (st == IDB_OK) {
         std::lock_guard<std::mutex> lk(ix->mu);

@@ -183,6 +183,52 @@ __device__ __forceinline__ float batch_butterfly(float (&p)[NB], int lane) {
     return p[0];
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Cosine distance (DESIGN.md §3a): the canonical squared L2 between canonically normalised rows; the caller is told half of it.
+// ---------------------------------------------------------------------------------------------------------
+enum Metric : uint32_t { kMetricL2Sq = 0, kMetricCosine = 1 };  // = IDB_METRIC_*
+
+// Chunk c of a row of `dim` elements at any alignment (zeros beyond the row).
+__device__ __forceinline__ float4 load_chunk_any(const float* row, uint32_t dim, uint32_t c) {
+    const uint32_t e = 4 * c;
+    return make_float4(e < dim ? row[e] : 0.f, e + 1 < dim ? row[e + 1] : 0.f, e + 2 < dim ? row[e + 2] : 0.f, e + 3 < dim ? row[e + 3] : 0.f);
+}
+
+// The ONE statement of the canonical normalisation, x^ = x / sqrt_rn(s): s = the canonical sum of squares, i.e. the §3 order
+// against a zero row (x - 0 == x for every float) in its long-row form — groups of 32 chunks in ascending order carrying the four
+// chains, lane_sum, butterfly_sum — then __fsqrt_rn and __fdiv_rn, both correctly rounded.  s == 0: the row stays all zeros;
+// s == inf: zeros and NaN (the IEEE result).  A NaN result is written as 0x7fc00000 (the GPU's and the CPU's divide return different
+// NaN encodings).  The whole warp calls it.  src: `dim` elements, any alignment; dst: `nchunks` chunks, zero padded.  dst may
+// alias src: every lane reads its own chunks before it writes them.
+__device__ __forceinline__ float canon_nan(float v) { return isnan(v) ? __int_as_float(0x7fc00000) : v; }
+__device__ __forceinline__ void normalize_row(const float* src, uint32_t dim, float4* dst, uint32_t nchunks, int lane) {
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 acc = zero;
+    for (uint32_t c = lane; c < nchunks; c += 32) l2_step(acc, load_chunk_any(src, dim, c), zero);
+    const float s = butterfly_sum(lane_sum(acc));
+    const float r = __fsqrt_rn(s);
+    for (uint32_t c = lane; c < nchunks; c += 32) {
+        const float4 x = load_chunk_any(src, dim, c);
+        const uint32_t e = 4 * c;
+        float4 y = zero;
+        if (s != 0.f) {
+            y.x = canon_nan(__fdiv_rn(x.x, r));  // (element e < dim always: c < nchunks)
+            y.y = e + 1 < dim ? canon_nan(__fdiv_rn(x.y, r)) : 0.f;
+            y.z = e + 2 < dim ? canon_nan(__fdiv_rn(x.z, r)) : 0.f;
+            y.w = e + 3 < dim ? canon_nan(__fdiv_rn(x.w, r)) : 0.f;
+        }
+        dst[c] = y;
+    }
+}
+
+// What the caller is told for a key's canonical distance bits.  Squared L2: the distance itself.  Cosine: 0.5 * ‖x^ - y^‖² =
+// 1 - cos (exact for normal floats), NaN written as the canonical 0x7fc00000 (a multiply would return 0x7fffffff), +inf stays +inf.
+__device__ __forceinline__ float reported_distance(uint32_t dbits, uint32_t metric) {
+    const float d = __uint_as_float(dbits);
+    if (metric == kMetricL2Sq) return d;
+    return dbits == 0x7fc00000u ? d : __fmul_rn(0.5f, d);
+}
+
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 __device__ __forceinline__ uint32_t canon_bits(float d) {

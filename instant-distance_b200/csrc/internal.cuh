@@ -60,6 +60,7 @@ struct SearchArgs {
     uint64_t* out_keys;                // optional: nq x k packed (distance bits << 32 | id_map[pid]) for the sharded all-gather
     const uint32_t* id_map;            // optional: PointId -> caller's global row id
     int variant;                       // tuning variant of the kernel template (0 = default)
+    uint32_t metric;                   // Metric: how out_dist reports a key's distance (out_keys always carry the key's own bits)
 };
 
 // Persisting-L2 access-policy window attached to a launch (the b16 visited tables), or none.
@@ -117,6 +118,7 @@ struct Lane {
     uint32_t* fail_list = nullptr; size_t fail_cap = 0;
     uint32_t* counters = nullptr; size_t counters_cap = 0;
     float* q = nullptr;           size_t q_cap = 0;
+    float* qn = nullptr;          size_t qn_cap = 0;   // a cosine call's normalised queries (K1 and its retry pass read them)
     uint32_t* ids = nullptr;      size_t ids_cap = 0;
     float* dist = nullptr;        size_t dist_cap = 0;
     uint32_t* len = nullptr;      size_t len_cap = 0;
@@ -174,6 +176,7 @@ struct Index {
     float* d_points = nullptr;                 // n x nchunks*4 f32 (PointId order); null when the rows are stored as bf16
     uint16_t* d_points_bf16 = nullptr;         // n x nchunks*4 bf16 (storage = IDB_STORAGE_BF16)
     bool bf16 = false;
+    uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
     uint32_t* d_zero = nullptr;                // n x 2M
     std::vector<uint32_t*> d_upper;            // [l-1] -> n_l x M
     std::vector<uint64_t> upper_n;
@@ -212,12 +215,18 @@ struct Index {
     // because profilers that replay a kernel (ncu) re-launch it without its launch attributes.
     idb_status attach_window(Lane& ln, const LaunchWindow& win);
     idb_status ensure_lane_scratch(Lane& ln, uint64_t nq);
-    idb_status enqueue_search(Lane& ln, const float* d_queries_padded, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
+    // d_queries: q_stride floats per row.  An L2 index takes them as K1 reads them (q_stride = nchunks * 4, zero padded, 16-byte
+    // aligned); a cosine index normalises them into the lane's buffer first (any q_stride >= dim, any alignment).
+    idb_status enqueue_search(Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
                               float* d_dist, uint32_t* d_len, uint64_t* out_keys);
     Lane& pick_lane();
 };
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
+// normalize_rows_kernel: dst[r] (nchunks * 4 floats, zero padded) = the canonical normalisation of src[r] (src_stride floats per row,
+// dim used, any alignment), one warp per row.  dst may equal src when src_stride == nchunks * 4.
+cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,
+                           cudaStream_t st);
 cudaError_t ensure_u32(uint32_t*& p, size_t& cap, size_t need);
 cudaError_t ensure_u64(uint64_t*& p, size_t& cap, size_t need);
 cudaError_t ensure_f32(float*& p, size_t& cap, size_t need);

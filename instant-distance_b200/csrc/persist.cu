@@ -5,6 +5,7 @@
 // other (dim, M) use the same scheme.  The layout is restated from bincode's documented encoding — no reference-written
 // fixture exists in the reference tree, so byte-level parity with a real file is UNPINNED (DESIGN.md §7).
 // An `HnswMap` file continues with `values` (lib.rs:131-134): idb_index_load reports the offset where they start.
+// The file does not record the metric: a cosine index saves its (normalised) rows, and idb_index_load_ex takes them as given.
 #include <cstdio>
 #include <cstring>
 #include <vector>
@@ -67,9 +68,15 @@ idb_status idb_index_save(const idb_index* index, const char* path) {
 }
 
 idb_status idb_index_load(const char* path, uint32_t dim, uint32_t M, int32_t device, idb_index** out_index, uint64_t* out_values_offset) {
+    return idb_index_load_ex(path, dim, M, IDB_METRIC_L2SQ, device, out_index, out_values_offset);
+}
+
+idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M, uint32_t metric, int32_t device, idb_index** out_index,
+                             uint64_t* out_values_offset) {
     if (!path || !out_index) return fail(IDB_ERR_INVALID_ARG, "null argument");
     *out_index = nullptr;
     if (dim == 0 || M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "dim/M invalid");
+    if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
     File in;
     in.f = std::fopen(path, "rb");
     if (!in.f) return fail(IDB_ERR_IO, "cannot open %s", path);
@@ -99,9 +106,10 @@ idb_status idb_index_load(const char* path, uint32_t dim, uint32_t M, int32_t de
     if (out_values_offset) *out_values_offset = (uint64_t)std::ftell(in.f);
     for (uint32_t v : zero)
         if (v != IDB_INVALID && v >= n) return fail(IDB_ERR_FORMAT, "%s: adjacency refers to PointId %u >= %llu", path, v, (unsigned long long)n);
-    // the same checks as for any adopted graph (entries inside their layer, n >= n_1 >= ... >= 1); a file that fails them is malformed
-    const idb_status st = idb_index_from_graph_f32(pts.data(), n, dim, M, (uint32_t)std::min<uint64_t>(ef, 0xFFFFFFFFu), zero.data(),
-                                                   (uint32_t)nl, ptrs.data(), counts.data(), device, out_index);
+    // the same checks as for any adopted graph (entries inside their layer, n >= n_1 >= ... >= 1; for cosine, unit rows); a file that
+    // fails them is malformed
+    const idb_status st = idb_index_from_graph_ex(pts.data(), n, dim, M, (uint32_t)std::min<uint64_t>(ef, 0xFFFFFFFFu), zero.data(),
+                                                  (uint32_t)nl, ptrs.data(), counts.data(), IDB_STORAGE_F32, metric, device, out_index);
     return st == IDB_ERR_INVALID_ARG ? IDB_ERR_FORMAT : st;
 }
 

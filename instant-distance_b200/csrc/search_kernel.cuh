@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(kSearchWarps * 32, OCC) search_kernel(SearchAr
             const uint32_t gid = j < len ? (a.id_map ? a.id_map[key_pid(key)] : key_pid(key)) : kInvalid;
             a.out_ids[qi * a.k + j] = gid;
             if (a.out_keys) a.out_keys[qi * a.k + j] = j < len ? (((uint64_t)key_dbits(key) << 32) | gid) : kKeyNone;
-            if (a.out_dist) a.out_dist[qi * a.k + j] = j < len ? __uint_as_float(key_dbits(key)) : __int_as_float(0x7f800000);
+            if (a.out_dist) a.out_dist[qi * a.k + j] = j < len ? reported_distance(key_dbits(key), a.metric) : __int_as_float(0x7f800000);
         }
         if (lane == 0) {
             if (a.out_len) a.out_len[qi] = len;

@@ -58,8 +58,9 @@ NcclApi& nccl() {
 // Keys are unique (global ids are), so rank(key) = #{keys smaller} is a permutation.  The lists are NOT assumed sorted by
 // the full key: a shard orders exact-distance ties by its local PointId, the merged order is by global id.
 // out_keys != null: write the merged keys (the local pre-merge of a rank that holds several shards) instead of ids / distances.
+// The keys carry the traversal's own distance bits; out_dist reports them through reported_distance (the shards' metric).
 __global__ void merge_topk_kernel(const uint64_t* all_keys /* G x nq x k */, uint32_t G, uint64_t nq, uint32_t k,
-                                  uint32_t* out_ids, float* out_dist, uint32_t* out_len, uint64_t* out_keys) {
+                                  uint32_t* out_ids, float* out_dist, uint32_t* out_len, uint64_t* out_keys, uint32_t metric) {
     extern __shared__ uint64_t sm_keys[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     uint64_t* keys = sm_keys + (size_t)warp * G * k;
@@ -80,7 +81,7 @@ __global__ void merge_topk_kernel(const uint64_t* all_keys /* G x nq x k */, uin
                 if (out_keys) out_keys[q * k + rank] = key;
                 else {
                     out_ids[q * k + rank] = (uint32_t)key;
-                    if (out_dist) out_dist[q * k + rank] = __uint_as_float((uint32_t)(key >> 32));
+                    if (out_dist) out_dist[q * k + rank] = reported_distance((uint32_t)(key >> 32), metric);
                 }
             }
         }
@@ -185,7 +186,7 @@ static idb_status launch_merge(Index* ix, cudaStream_t st, const uint64_t* keys,
     const size_t smem = (size_t)wpb * per_warp;
     if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(merge_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const unsigned grid = (unsigned)std::min<uint64_t>((nq + wpb - 1) / wpb, (uint64_t)ix->num_sms * 8);
-    merge_topk_kernel<<<grid, wpb * 32, smem, st>>>(keys, G, nq, k, d_ids, d_dist, d_len, d_keys);
+    merge_topk_kernel<<<grid, wpb * 32, smem, st>>>(keys, G, nq, k, d_ids, d_dist, d_len, d_keys, ix->metric);
     CUDA_TRY(cudaGetLastError());
     return IDB_OK;
 }
@@ -239,7 +240,8 @@ static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, 
     NCCL_TRY(nccl().AllGather(ln.keys_local, ln.keys_all, per, ncclUint64, c->comm, ln.stream));
     st = launch_merge(ix, ln.stream, ln.keys_all, (uint32_t)c->world, nq, k, d_out_ids, d_out_dist, d_out_len, nullptr, max_smem);
     if (st != IDB_OK) return st;
-    ln.last_launches = 2 * n_local + (n_local > 1 ? 1 : 0) + 2;  // K1 + retry per shard, pre-merge, all-gather, merge
+    // (query normalisation) + K1 + retry per shard, pre-merge, all-gather, merge
+    ln.last_launches = (ix->metric == kMetricCosine ? 3 : 2) * n_local + (n_local > 1 ? 1 : 0) + 2;
     return IDB_OK;
 }
 
@@ -253,8 +255,11 @@ struct ShardLocks {
         for (uint32_t i = 0; i < n; ++i) {
             Index* ix = reinterpret_cast<Index*>(shards[i]);
             if (!ix) return fail(IDB_ERR_INVALID_ARG, "shard %u is null", i);
-            if (ix->device != reinterpret_cast<Index*>(shards[0])->device || ix->dim != reinterpret_cast<Index*>(shards[0])->dim)
+            const Index* first = reinterpret_cast<Index*>(shards[0]);
+            if (ix->device != first->device || ix->dim != first->dim)
                 return fail(IDB_ERR_INVALID_ARG, "shard %u: all shards of a rank must live on one device and have one dim", i);
+            if (ix->metric != first->metric)  // their keys would not be comparable
+                return fail(IDB_ERR_INVALID_ARG, "shard %u: all shards of a call must have one metric", i);
             v.push_back(ix);
         }
         std::sort(v.begin(), v.end());

@@ -5,7 +5,9 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
   * points may have any dimension (the reference fixes DIMENSIONS = 300, py:448, and zero-pads shorter inputs, py:367-374;
     here every point of an index is zero-padded to the longest point given at build time, and a longer query raises the
     same `TypeError("point array too long")`, py:369-370);
-  * `Hnsw.search_many / HnswMap.search_many` expose the batched search the GPU is built for.
+  * `Hnsw.search_many / HnswMap.search_many` expose the batched search the GPU is built for;
+  * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
+    DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it.
 """
 import ctypes as C
 import random
@@ -35,9 +37,10 @@ class Config:
         self.ml = float(p.ml)
         self.seed = random.getrandbits(64)
         self.heuristic = Heuristic()
+        self.metric = "l2sq"  # or "cosine"
 
     def _params(self):
-        kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed)
+        kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed, metric=self.metric)
         if self.heuristic is None:
             kw["heuristic"] = 0
         else:
@@ -122,10 +125,10 @@ class Hnsw:
         self._ix.save(fname)
 
     @staticmethod
-    def load(fname, dim=300, M=32):
-        """py:121-129.  The file does not store dim / M (fixed arrays in the reference: 300 / 32)."""
+    def load(fname, dim=300, M=32, metric="l2sq"):
+        """py:121-129.  The file does not store dim / M (fixed arrays in the reference: 300 / 32), nor the metric."""
         try:
-            ix, _ = _abi.Index.load(fname, dim, M)
+            ix, _ = _abi.Index.load(fname, dim, M, metric=metric)
         except _abi.IdbError as e:
             if e.status == _abi.ERR_IO:
                 raise OSError(str(e)) from e
@@ -162,12 +165,12 @@ class HnswMap(Hnsw):
                 f.write(struct.pack("<IQ", 0, len(b)) + b)
 
     @staticmethod
-    def load(fname, dim=300, M=32):
+    def load(fname, dim=300, M=32, metric="l2sq"):
         """py:58-67."""
         import struct
 
         try:
-            ix, off = _abi.Index.load(fname, dim, M)
+            ix, off = _abi.Index.load(fname, dim, M, metric=metric)
         except _abi.IdbError as e:
             if e.status == _abi.ERR_IO:
                 raise OSError(str(e)) from e

@@ -23,6 +23,7 @@ SYMBOLS = [
     "idb_index_stream", "idb_index_sync", "idb_index_free",
     "idb_comm_unique_id", "idb_comm_create", "idb_comm_free", "idb_index_set_id_map", "idb_sharded_search_batch_f32",
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
+    "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
 ]
 
 
@@ -66,6 +67,12 @@ def lib():
     L.idb_index_from_graph_f32.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_uint32,
                                            C.POINTER(u32p), u64p, C.c_int32, C.POINTER(vp)]
     L.idb_index_from_graph_bf16.argtypes = L.idb_index_from_graph_f32.argtypes
+    L.idb_build_ex.argtypes = [f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), C.c_uint32, C.POINTER(vp), u32p]
+    L.idb_index_from_graph_ex.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_uint32,
+                                          C.POINTER(u32p), u64p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp)]
+    L.idb_index_load_ex.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
+    L.idb_normalize_f32.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_int32, f32p]
+    L.idb_index_metric.argtypes = [vp, u32p]
     L.idb_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.c_uint32, u32p, f32p, u32p]
     L.idb_search_batch_device.argtypes = [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, vp]
     L.idb_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, vp]
@@ -130,6 +137,13 @@ def ptr(a, t):
 
 
 STORAGE = {"f32": 0, "bf16": 1}
+METRIC = {"l2sq": 0, "cosine": 1}  # IDB_METRIC_*: squared L2, or 1 - cos through canonically normalised rows (DESIGN.md §3a)
+
+
+def _metric(metric):
+    if metric not in METRIC:
+        raise ValueError(f"metric must be one of {sorted(METRIC)}, not {metric!r}")
+    return METRIC[metric]
 PROGRESS_FN = C.CFUNCTYPE(None, C.c_uint64, C.c_uint64, C.c_void_p)
 
 
@@ -163,21 +177,21 @@ class Index:
             pass
 
     @classmethod
-    def from_graph(cls, points, zero, upper, M, ef_search=100, device=0, storage="f32"):
+    def from_graph(cls, points, zero, upper, M, ef_search=100, device=0, storage="f32", metric="l2sq"):
+        """metric="cosine": the points are taken as given and must be unit rows (or all zeros) — see normalize()."""
         points, zero = f32(points), np.ascontiguousarray(zero, dtype=np.uint32)
         n, dim = points.shape
         ups = [np.ascontiguousarray(u, dtype=np.uint32) for u in upper]
         arr = (C.POINTER(C.c_uint32) * max(1, len(ups)))(*[ptr(u, C.c_uint32) for u in ups])
         un = np.array([u.shape[0] for u in ups] or [0], dtype=np.uint64)
         h = C.c_void_p()
-        fn = lib().idb_index_from_graph_bf16 if storage == "bf16" else lib().idb_index_from_graph_f32
-        check(fn(ptr(points, C.c_float), n, dim, M, ef_search, ptr(zero, C.c_uint32), len(ups),
-                                             arr, ptr(un, C.c_uint64), device, C.byref(h)))
+        check(lib().idb_index_from_graph_ex(ptr(points, C.c_float), n, dim, M, ef_search, ptr(zero, C.c_uint32), len(ups), arr,
+                                            ptr(un, C.c_uint64), STORAGE[storage], _metric(metric), device, C.byref(h)))
         return cls(h)
 
     @classmethod
-    def build(cls, rows, progress=None, **kw):
-        """progress: optional callable(done, total) — Builder::progress (lib.rs:70-75)."""
+    def build(cls, rows, progress=None, metric="l2sq", **kw):
+        """progress: optional callable(done, total) — Builder::progress (lib.rs:70-75).  metric: "l2sq" or "cosine"."""
         rows = f32(rows)
         n, dim = rows.shape
         p = default_params(**kw)
@@ -187,23 +201,29 @@ class Index:
             p.progress = C.cast(cb, C.c_void_p)
         ids = np.empty(n, dtype=np.uint32)
         h = C.c_void_p()
-        check(lib().idb_build_f32(ptr(rows, C.c_float), n, dim, C.byref(p), C.byref(h), ptr(ids, C.c_uint32)))
+        check(lib().idb_build_ex(ptr(rows, C.c_float), n, dim, C.byref(p), _metric(metric), C.byref(h), ptr(ids, C.c_uint32)))
         return cls(h), ids
 
     def save(self, path):
         check(lib().idb_index_save(self._h, os.fsencode(path)))
 
     @classmethod
-    def load(cls, path, dim=300, M=32, device=0):
-        """Returns (Index, offset of the HnswMap values in the file)."""
+    def load(cls, path, dim=300, M=32, device=0, metric="l2sq"):
+        """Returns (Index, offset of the HnswMap values in the file).  The file does not record the metric."""
         h, off = C.c_void_p(), C.c_uint64()
-        check(lib().idb_index_load(os.fsencode(path), dim, M, device, C.byref(h), C.byref(off)))
+        check(lib().idb_index_load_ex(os.fsencode(path), dim, M, _metric(metric), device, C.byref(h), C.byref(off)))
         return cls(h), int(off.value)
 
     def info(self):
         i = Info()
         check(lib().idb_index_info(self._h, C.byref(i)))
         return i
+
+    @property
+    def metric(self):
+        m = C.c_uint32()
+        check(lib().idb_index_metric(self._h, C.byref(m)))
+        return {v: k for k, v in METRIC.items()}[int(m.value)]
 
     def _queries(self, queries):
         """n x dim f32 matrix; narrower rows are zero-padded like the reference pads short points (py:363-375), wider ones rejected."""
@@ -364,6 +384,16 @@ def sharded_search_multi(shards, comm, queries, ef_search=0, k=10):
 def sharded_search_multi_device(shards, comm, d_queries, nq, ef_search, k, d_ids, d_dist, d_len):
     """Device pointers; enqueues on lane 0 of shards[0] (every shard's stream is joined into it) and returns."""
     check(lib().idb_sharded_search_batch_device_multi(_handles(shards), len(shards), comm._h, d_queries, nq, ef_search, k, d_ids, d_dist, d_len))
+
+
+def normalize(rows, device=0):
+    """The canonical normalisation of every row on the device (idb_normalize_f32): what a cosine index stores for them."""
+    rows = f32(rows)
+    if rows.ndim == 1:
+        rows = rows[None, :]
+    out = np.empty_like(rows)
+    check(lib().idb_normalize_f32(ptr(rows, C.c_float), rows.shape[0], rows.shape[1], device, ptr(out, C.c_float)))
+    return out
 
 
 def distance(a, b, device=0):

@@ -28,6 +28,13 @@ struct IdbIndex {
 extern "C" {
     fn idb_params_default(p: *mut IdbParams) -> i32;
     fn idb_build_f32(rows: *const f32, n: u64, dim: u32, p: *const IdbParams, out: *mut *mut IdbIndex, out_ids: *mut u32) -> i32;
+    fn idb_build_ex(rows: *const f32, n: u64, dim: u32, p: *const IdbParams, metric: u32, out: *mut *mut IdbIndex, out_ids: *mut u32) -> i32;
+    fn idb_index_from_graph_ex(points: *const f32, n: u64, dim: u32, m: u32, ef_search: u32, zero: *const u32, n_upper: u32,
+                               upper: *const *const u32, upper_n: *const u64, storage: u32, metric: u32, device: i32,
+                               out: *mut *mut IdbIndex) -> i32;
+    fn idb_index_load_ex(path: *const c_char, dim: u32, m: u32, metric: u32, device: i32, out: *mut *mut IdbIndex, values_offset: *mut u64) -> i32;
+    fn idb_normalize_f32(rows: *const f32, n: u64, dim: u32, device: i32, out: *mut f32) -> i32;
+    fn idb_index_metric(ix: *const IdbIndex, out: *mut u32) -> i32;
     fn idb_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, ef: u32, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
     fn idb_index_free(ix: *mut IdbIndex);
     fn idb_last_error() -> *const c_char;
@@ -59,6 +66,19 @@ impl Point for F32Point {
     fn distance(&self, o: &Self) -> f32 { self.0.iter().zip(&o.0).map(|(a, b)| (a - b) * (a - b)).sum() }
 }
 
+/// What the index reports (include/instant_distance_b200.h IDB_METRIC_*): squared L2, or 1 - cos through canonically normalised
+/// points and queries (DESIGN.md §3a).  `F32Point::distance` stays squared L2.
+pub const METRIC_L2SQ: u32 = 0;
+pub const METRIC_COSINE: u32 = 1;
+
+/// The canonical normalisation the cosine metric applies, evaluated on `device` (rows: n x dim, row-major).
+pub fn normalize(rows: &[f32], dim: usize, device: i32) -> Vec<f32> {
+    let mut out = vec![0f32; rows.len()];
+    let rc = unsafe { idb_normalize_f32(rows.as_ptr(), (rows.len() / dim.max(1)) as u64, dim as u32, device, out.as_mut_ptr()) };
+    assert_eq!(rc, 0, "{}", last_error());
+    out
+}
+
 /// lib.rs:115-128
 #[derive(Copy, Clone, Debug)]
 pub struct Heuristic { pub extend_candidates: bool, pub keep_pruned: bool }
@@ -68,15 +88,17 @@ impl Default for Heuristic {
 
 /// lib.rs:21-113
 #[derive(Clone)]
-pub struct Builder { ef_search: usize, ef_construction: usize, heuristic: Option<Heuristic>, ml: f32, seed: u64 }
+pub struct Builder { ef_search: usize, ef_construction: usize, heuristic: Option<Heuristic>, ml: f32, seed: u64, metric: u32 }
 impl Default for Builder {
     fn default() -> Self {
         let mut p = unsafe { std::mem::zeroed::<IdbParams>() };
         unsafe { idb_params_default(&mut p) };
-        Self { ef_search: 100, ef_construction: 100, heuristic: Some(Heuristic::default()), ml: p.ml, seed: 0 }
+        Self { ef_search: 100, ef_construction: 100, heuristic: Some(Heuristic::default()), ml: p.ml, seed: 0, metric: METRIC_L2SQ }
     }
 }
 impl Builder {
+    /// Not in the reference: METRIC_L2SQ (default) or METRIC_COSINE.
+    pub fn metric(mut self, v: u32) -> Self { self.metric = v; self }
     pub fn ef_construction(mut self, v: usize) -> Self { self.ef_construction = v; self }
     pub fn ef_search(mut self, v: usize) -> Self { self.ef_search = v; self }
     pub fn select_heuristic(mut self, h: Option<Heuristic>) -> Self { self.heuristic = h; self }
@@ -96,7 +118,7 @@ impl Builder {
         if let Some(h) = self.heuristic { p.extend_candidates = h.extend_candidates as i32; p.keep_pruned = h.keep_pruned as i32; }
         let mut raw = std::ptr::null_mut();
         let mut ids = vec![0u32; points.len()];
-        let rc = unsafe { idb_build_f32(flat.as_ptr(), points.len() as u64, dim as u32, &p, &mut raw, ids.as_mut_ptr()) };
+        let rc = unsafe { idb_build_ex(flat.as_ptr(), points.len() as u64, dim as u32, &p, self.metric, &mut raw, ids.as_mut_ptr()) };
         assert_eq!(rc, 0, "{}", last_error()); // the reference's build is infallible
         let mut shuffled = points.clone(); // Hnsw::points is in PointId order (lib.rs:263-270)
         for (orig, pid) in ids.iter().enumerate() { shuffled[*pid as usize] = points[orig].clone(); }
