@@ -158,6 +158,11 @@ IDB_API idb_status idb_last_search_failures(idb_index* index, uint32_t lane, uin
  * re-run by the retry pass (their results are valid; a persistently non-zero figure costs throughput, and the library then switches the
  * index to its larger, DRAM-resident visited flavour by itself).  lane = 0xFFFFFFFF: the lane the last call on this index used. */
 IDB_API idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint32_t* out_retried);
+/* Diagnostics: how many candidate rows the last call on `lane` fetched in full, over all its queries (and its retry pass).  Without
+ * screening that is the sum of the per-query distance counters; with it (the default, DESIGN §4) the rows whose 8-bit-code lower bound
+ * already proves they would not be admitted are not fetched, so it is smaller.  Results are the same either way.
+ * lane = 0xFFFFFFFF: the lane the last call on this index used. */
+IDB_API idb_status idb_last_search_full_fetches(idb_index* index, uint32_t lane, uint64_t* out_rows);
 /* enabled = 1: reserve persisting L2 for the visited tables on `device` (see idb_search_batch_f32).  enabled = 0 (the default):
  * this library never touches the device's persisting-L2 limit nor attaches access-policy windows on `device`. */
 IDB_API idb_status idb_device_set_persisting_l2(int32_t device, int32_t enabled);
@@ -211,6 +216,11 @@ IDB_API idb_status idb_debug_gather_bench(idb_index* index, uint32_t n_items, ui
  * wait for them (K1's dependency).  *out_bytes counts the ROW bytes only, like K1's algorithmic bytes. */
 IDB_API idb_status idb_debug_gather_mix_bench(idb_index* index, uint32_t n_items, uint32_t batches, uint32_t chain, uint32_t reps,
                                               uint32_t atomics_per_batch, uint32_t mode, float* out_ms, double* out_bytes);
+/* Measurement / test only: for each pair (query index, PointId) of `pairs` (npairs x 2), the screening bound K1 compares with the
+ * furthest distance and the canonical distance (queries: nq x dim f32, used as given).  IDB_ERR_UNSUPPORTED when the index has no
+ * screening table (IDB_SCREEN=0, an empty index, a non-finite stored value, or rows of more than 1024 elements). */
+IDB_API idb_status idb_debug_screen_bound(idb_index* index, const float* queries, uint64_t nq, const uint32_t* pairs, uint64_t npairs,
+                                          float* out_bound, float* out_dist);
 
 IDB_API void* idb_index_stream(idb_index* index);      /* lane 0's cudaStream_t: builds, uploads and idb_search_batch_device run on it */
 IDB_API idb_status idb_index_sync(idb_index* index);   /* cudaStreamSynchronize on every lane of the index */

@@ -527,6 +527,7 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     a.variant = variant;
     a.out_keys = out_keys;
     a.id_map = d_id_map;
+    a.full_tally = reinterpret_cast<unsigned long long*>(ln.ctrl + 8);  // K1 and the retry pass both add to it
 
     const int ch = (int)((nchunks + 31) / 32);
     if (ch > 8 && (nchunks + 31) / 32 * 512 > 40 * 1024)
@@ -620,6 +621,8 @@ GraphView Index::view() const {
     g.M = M;
     g.n = n;
     g.flags = opt_flags;
+    g.codes = d_codes;
+    g.cparams = d_cparams;
     return g;
 }
 
@@ -629,6 +632,8 @@ Index::~Index() {
         if (ln.stream) cudaStreamSynchronize(ln.stream);
     cudaFree(d_points);
     cudaFree(d_points_bf16);
+    cudaFree(d_codes);
+    cudaFree(d_cparams);
     cudaFree(d_zero);
     for (auto* p : d_upper) cudaFree(p);
     cudaFree(d_upper_ptrs);
@@ -662,6 +667,7 @@ idb_status Index::init_device(int dev) {
     if (const char* e = std::getenv("IDB_B16_CAP")) b16_cap_16ths = (uint32_t)std::min(14, std::max(1, std::atoi(e)));
     if (const char* e = std::getenv("IDB_B16_BYTES")) b16_bytes_override = (uint32_t)std::max(64, std::atoi(e));
     if (const char* e = std::getenv("IDB_VIS_SLOTS")) vis_slots_override = next_pow2((uint64_t)std::max(64, std::atoi(e)));
+    if (const char* e = std::getenv("IDB_SCREEN")) screen = std::atoi(e) != 0;
     return IDB_OK;
 }
 
@@ -807,6 +813,7 @@ idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint32_t dim
     idb_status st = ix->init_device(device);
     if (st == IDB_OK) st = ix->upload(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n);
     if (st == IDB_OK && storage == IDB_STORAGE_BF16) st = ix->narrow_points_to_bf16();
+    if (st == IDB_OK) st = ix->build_codes();
     if (st != IDB_OK) { delete ix; return st; }
     *out_index = reinterpret_cast<idb_index*>(ix);
     return IDB_OK;

@@ -402,6 +402,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
     if (st == IDB_OK) {
         std::lock_guard<std::mutex> lk(ix->mu);
         st = build_index(ix, rows, n, dim, *params, out_ids);
+        if (st == IDB_OK) st = ix->build_codes();  // from the final stored rows (normalised, narrowed); the build itself does not screen
     }
     if (st != IDB_OK) { delete ix; return st; }
     *out_index = reinterpret_cast<idb_index*>(ix);

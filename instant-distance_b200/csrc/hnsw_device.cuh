@@ -46,6 +46,9 @@ struct GraphView {
     uint64_t n;
     uint32_t flags;              // kOpt* tuning switches (never change results)
     uint32_t bf16;               // rows are stored as bf16 (BASELINE config 4's data format); arithmetic stays fp32
+    // Screening table (DESIGN §2, §4), or null: K1 then fetches every candidate row in full.
+    const uint32_t* codes;       // n rows of nchunks u32: word c holds the 8-bit codes of elements 4c..4c+3 (byte k = element 4c+k)
+    const float4* cparams;       // 3 x nchunks float4: per element scale, offset, E (x~ = fmaf(code, scale, offset), |x - x~| <= E)
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -164,7 +167,10 @@ __device__ __forceinline__ float butterfly_sum(float s) {
 // log2(NB) stages are "transposing" (each lane hands half of its values to its partner and keeps the other half,
 // split by even/odd index), so NB vectors cost NB-1 shuffles instead of 5*NB; the remaining stages are plain.
 // Same add tree as butterfly_sum for every vector.  On return lane l holds the total of vector (l & (NB-1)).
-template <int NB>
+// kDown: every add rounds toward -inf instead (the screening bound, which must never exceed the exact sum).
+template <bool kDown>
+__device__ __forceinline__ float fadd_dir(float a, float b) { return kDown ? __fadd_rd(a, b) : __fadd_rn(a, b); }
+template <int NB, bool kDown = false>
 __device__ __forceinline__ float batch_butterfly(float (&p)[NB], int lane) {
     int off = 1;
 #pragma unroll
@@ -174,12 +180,12 @@ __device__ __forceinline__ float batch_butterfly(float (&p)[NB], int lane) {
         for (int i = 0; i < m / 2; ++i) {
             float send = up ? p[2 * i] : p[2 * i + 1];
             float keep = up ? p[2 * i + 1] : p[2 * i];
-            p[i] = __fadd_rn(keep, __shfl_xor_sync(kFullMask, send, off));
+            p[i] = fadd_dir<kDown>(keep, __shfl_xor_sync(kFullMask, send, off));
         }
         off <<= 1;
     }
 #pragma unroll
-    for (int o = NB; o <= 16; o <<= 1) p[0] = __fadd_rn(p[0], __shfl_xor_sync(kFullMask, p[0], o));
+    for (int o = NB; o <= 16; o <<= 1) p[0] = fadd_dir<kDown>(p[0], __shfl_xor_sync(kFullMask, p[0], o));
     return p[0];
 }
 
@@ -576,6 +582,7 @@ struct WarpState {
     uint32_t ntie;
     uint32_t status;
     uint32_t n_expand, n_dist;   // per-layer instrumentation (SURVEY §8d counters)
+    uint32_t n_full;             // rows fetched in full over the whole descent (n_dist minus what the screen dropped)
     VisitedSet vis;
 };
 
@@ -677,6 +684,94 @@ __device__ __forceinline__ void batch_distances(const GraphView& g, const QVec<C
                                                 uint32_t n_new, int lane) {
     if constexpr (CH == 0) batch_distances_long<kLongRowsInFlight, RT>(g, q, cpid, ckey, n_new, lane);
     else batch_distances_impl<CH, NB, FULL, RT>(g, q.r, cpid, ckey, n_new, lane);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Screening (DESIGN §4 "screen"): a lower bound of a candidate's canonical distance from its 8-bit codes (128 B per row at dim 128
+// instead of 512 B), so that rows the admission test would reject anyway are never fetched in full.
+//   x~_i = fmaf(code_i, scale_i, offset_i) (round to nearest), E_i >= |x_i - x~_i| over every stored row;
+//   a_i  = max(0, |q_i - x~_i|_rz - E_i)_rd <= |q_i - x_i|,   LB = sum_rd a_i^2 <= sum (q_i - x_i)^2 (exact);
+//   bound = LB * (1 - 2^-16)_rd if that is > 2^-100, else 0.  bound > dist(furthest)  =>  canonical distance > dist(furthest).
+// The factor covers the canonical order's roundings (at most CH + 9 per term, CH <= 8), the floor its underflow; NaN bounds are 0.
+// ---------------------------------------------------------------------------------------------------------
+constexpr float kScreenKeep = 0.9999847412109375f;  // 1 - 2^-16, exact
+constexpr float kScreenFloor = 0x1p-100f;
+// Code byte k of w as a float, exactly: 0x4B0000cc is 2^23 + c.
+__device__ __forceinline__ float code_of(uint32_t w, int k) {
+    return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u | (uint32_t)k)), 8388608.f);
+}
+__device__ __forceinline__ float screen_term(float q, float code, float scale, float offset, float e, float acc) {
+    const float d = fabsf(__fsub_rz(q, __fmaf_rn(code, scale, offset)));  // <= |q - x~|
+    const float a = fmaxf(__fsub_rd(d, e), 0.f);                          // <= |q - x|  (a NaN query element gives 0)
+    return __fmaf_rd(a, a, acc);
+}
+// Scale / offset / E of chunk c (zeros beyond the row: those elements contribute 0).  Loaded per use, from L1: keeping them in
+// registers for all CH chunks would not fit next to the query.
+struct ScreenChunk {
+    float4 sc, of, er;
+};
+__device__ __forceinline__ ScreenChunk screen_chunk_params(const GraphView& g, uint32_t c, bool ok) {
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    ScreenChunk p;
+    p.sc = ok ? __ldg(g.cparams + c) : z;
+    p.of = ok ? __ldg(g.cparams + g.nchunks + c) : z;
+    p.er = ok ? __ldg(g.cparams + 2 * g.nchunks + c) : z;
+    return p;
+}
+// acc + this lane's four terms of one chunk (query chunk q, code word w).
+__device__ __forceinline__ float screen_chunk(const float4& q, uint32_t w, const ScreenChunk& p, float acc) {
+    acc = screen_term(q.x, code_of(w, 0), p.sc.x, p.of.x, p.er.x, acc);
+    acc = screen_term(q.y, code_of(w, 1), p.sc.y, p.of.y, p.er.y, acc);
+    acc = screen_term(q.z, code_of(w, 2), p.sc.z, p.of.z, p.er.z, acc);
+    return screen_term(q.w, code_of(w, 3), p.sc.w, p.of.w, p.er.w, acc);
+}
+__device__ __forceinline__ float screen_finish(float lb) {
+    const float b = __fmul_rd(lb, kScreenKeep);
+    return b > kScreenFloor ? b : 0.f;
+}
+template <int CH>
+__device__ __forceinline__ constexpr int screen_rows() { return CH == 1 ? 32 : CH == 2 ? 16 : CH <= 4 ? 8 : 2; }  // code words in flight <= 32
+// Drops the candidates in cpid[0, n_new) whose bound exceeds fdist (the distance of the ef-th key of nearest) and compacts the rest,
+// in row order, to the front of cpid.  Returns how many are left.  Warp-uniform call.
+template <int CH, bool kFull>
+__device__ __forceinline__ uint32_t screen_candidates(const GraphView& g, const float4 (&q)[CH], uint32_t* cpid, uint32_t n_new, float fdist,
+                                                      int lane) {
+    constexpr int NS = screen_rows<CH>();
+    bool cok[CH];
+#pragma unroll
+    for (int j = 0; j < CH; ++j) cok[j] = kFull || (uint32_t)(lane + 32 * j) < g.nchunks;
+    const uint32_t* lane_codes = g.codes + lane;
+    uint32_t kept = 0;
+#pragma unroll 1
+    for (uint32_t b0 = 0; b0 < n_new; b0 += NS) {
+        const uint32_t nb = n_new - b0;
+        uint32_t w[NS][CH];
+#pragma unroll
+        for (int i = 0; i < NS; ++i) {
+            const bool ok = (uint32_t)i < nb;
+            const uint32_t* row = lane_codes + (size_t)cpid[b0 + i] * g.nchunks;  // (entries past n_new are stale ids: never loaded)
+#pragma unroll
+            for (int j = 0; j < CH; ++j) w[i][j] = (ok && cok[j]) ? __ldg(row + 32 * j) : 0u;
+        }
+        const uint32_t mine = (uint32_t)lane < (uint32_t)NS && (uint32_t)lane < nb ? cpid[b0 + lane] : kInvalid;
+        float p[NS];
+#pragma unroll
+        for (int i = 0; i < NS; ++i) p[i] = 0.f;
+#pragma unroll
+        for (int j = 0; j < CH; ++j) {
+            const ScreenChunk pc = screen_chunk_params(g, lane + 32 * j, cok[j]);
+#pragma unroll
+            for (int i = 0; i < NS; ++i) p[i] = screen_chunk(q[j], w[i][j], pc, p[i]);
+        }
+        const float bound = screen_finish(batch_butterfly<NS, true>(p, lane));  // lane l: row b0 + (l & (NS - 1))
+        const bool keep = mine != kInvalid && !(bound > fdist);
+        const uint32_t m = __ballot_sync(kFullMask, keep);
+        __syncwarp();  // every lane has read this batch's ids before any is overwritten (writes go to [kept, b0 + NS))
+        if (keep) cpid[kept + __popc(m & ((1u << lane) - 1u))] = mine;
+        kept += __popc(m);
+    }
+    __syncwarp();
+    return kept;
 }
 
 // EXPERIMENT — the TMA staging north_star describes: every point row of a batch is fetched by ONE cp.async.bulk (1-D bulk copy,
@@ -813,7 +908,8 @@ __device__ __forceinline__ void batch_distances_tma(const GraphView& g, const fl
 // kLive: rows may be rewritten concurrently (GPU build) -> read them through L2 (ld.global.cg), not the
 // read-only/L1 path.
 // ---------------------------------------------------------------------------------------------------------
-template <int CH, int ROW_T, int EF_T, int B, bool kLive, class RT, bool FULL, bool TMA = false>
+// SCREEN: compile the screening pass in (K1's register flavours); it runs when g.codes is set.
+template <int CH, int ROW_T, int EF_T, int B, bool kLive, class RT, bool FULL, bool TMA = false, bool SCREEN = false>
 __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, const QVec<CH>& q, const uint32_t* rows,
                                              uint32_t width, uint32_t links, uint32_t ef_cur, bool seed_entry, int lane) {
     const uint32_t lt_mask = (1u << lane) - 1;
@@ -919,7 +1015,16 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
             s.n_dist += n_new;
             if (n_new == 0) continue;
             __syncwarp();
+            // ---- screen (DESIGN §4): with nearest full, a candidate whose code bound exceeds the furthest distance has a key
+            // above the furthest key, so it would not be admitted; only the others are fetched in full, still in row order --------
+            if constexpr (SCREEN && CH > 0 && !kLive && !TMA) {
+                if (g.codes && s.cnt >= ef_cur) {
+                    n_new = screen_candidates<CH, FULL>(g, q.r, s.cpid, n_new, __uint_as_float(key_dbits(near[s.cnt - 1])), lane);
+                    if (n_new == 0) continue;
+                }
+            }
         }
+        s.n_full += n_new;
 
         // ---- distances (lib.rs:709-710) --------------------------------------------------------------------
         if constexpr (TMA) batch_distances_tma<CH, B>(g, q.r, s.cpid, s.ckey, n_new, lane, s);
@@ -1044,7 +1149,7 @@ __device__ __forceinline__ void cull(WarpState& s, int lane, bool next_big) {
 // Construction::insert's descent (lib.rs:443-463) when target_layer = the insert layer, ef_target = ef_construction.
 // Layers above the target are searched on the UpperNode snapshots with ef = 1; the target layer on the zero table.
 // On return nearest = (s.near_base + s.cur * s.near_len)[0..s.cnt).  counters (if non-null): {n_expand_upper, n_dist_upper, n_expand_target, n_dist_target}.
-template <int CH, int ROW_T, int EF_T, int B, bool kLive, class RT = RowF32, bool FULL = false, bool TMA = false>
+template <int CH, int ROW_T, int EF_T, int B, bool kLive, class RT = RowF32, bool FULL = false, bool TMA = false, bool SCREEN = false>
 __device__ __forceinline__ void descend(const GraphView& g, WarpState& s, const QVec<CH>& q, uint32_t target_layer,
                                         uint32_t ef_target, int lane, uint32_t* counters4) {
     s.cur = 0;
@@ -1053,6 +1158,7 @@ __device__ __forceinline__ void descend(const GraphView& g, WarpState& s, const 
     s.status = kQueryOk;
     s.n_expand = 0;
     s.n_dist = 0;
+    s.n_full = 0;
     s.vis.count = 0;
     s.vis.use_big = (g.n_upper == target_layer);  // no ef=1 layer above the target: go straight to the big tier
     uint32_t up_expand = 0, up_dist = 0;
@@ -1063,7 +1169,7 @@ __device__ __forceinline__ void descend(const GraphView& g, WarpState& s, const 
         const uint32_t* rows = above ? g.upper[cur - 1] : g.zero;
         const uint32_t width = above ? g.M : 2 * g.M;
         const uint32_t links = (above || target_layer != 0) ? g.M : 2 * g.M;  // lib.rs:445 / 366-369
-        search_layer<CH, ROW_T, EF_T, B, kLive, RT, FULL, TMA>(g, s, q, rows, width, links, above ? 1u : ef_target, seed, lane);
+        search_layer<CH, ROW_T, EF_T, B, kLive, RT, FULL, TMA, SCREEN>(g, s, q, rows, width, links, above ? 1u : ef_target, seed, lane);
         seed = false;
         if (!above || s.status != kQueryOk) break;
         cull<EF_T>(s, lane, /*next_big=*/(cur - 1 == target_layer));

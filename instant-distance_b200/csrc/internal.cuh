@@ -61,6 +61,7 @@ struct SearchArgs {
     const uint32_t* id_map;            // optional: PointId -> caller's global row id
     int variant;                       // tuning variant of the kernel template (0 = default)
     uint32_t metric;                   // Metric: how out_dist reports a key's distance (out_keys always carry the key's own bits)
+    unsigned long long* full_tally;    // optional: += rows fetched in full (the rows the screen did not drop), over the call
 };
 
 // Persisting-L2 access-policy window attached to a launch (the b16 visited tables), or none.
@@ -113,7 +114,7 @@ struct DeviceCtx {
 struct Lane {
     std::mutex mu;
     cudaStream_t stream = nullptr;
-    unsigned char* ctrl = nullptr;   // [0..8) K1 work counter, [16..20) K1 fail count, [32..40) retry work counter, [48..52) retry fail count
+    unsigned char* ctrl = nullptr;   // [0..8) K1 work counter, [8..16) rows fetched in full, [16..20) K1 fail count, [32..40) retry work counter, [48..52) retry fail count
     uint32_t* status = nullptr;   size_t status_cap = 0;
     uint32_t* fail_list = nullptr; size_t fail_cap = 0;
     uint32_t* counters = nullptr; size_t counters_cap = 0;
@@ -183,6 +184,11 @@ struct Index {
     const uint32_t** d_upper_ptrs = nullptr;   // device copy of the pointer table
     uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map)
     bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
+    // Screening table of the stored rows (DESIGN §2, §4): n x nchunks u32 of 8-bit codes + 3 x nchunks float4 (scale, offset, E).
+    // Null when screening is off (IDB_SCREEN=0), the index is empty, or a stored value is not finite.
+    uint32_t* d_codes = nullptr;
+    float4* d_cparams = nullptr;
+    bool screen = true;                        // IDB_SCREEN (default 1): build the table and let K1 screen with it; never changes results
 
     // tuning knobs (env IDB_OPT / IDB_VIS_MULT / IDB_VIS_TIER / IDB_B16_BYTES / IDB_VIS_SLOTS / IDB_VARIANT); none of them changes results
     uint32_t opt_flags = 0;       // L2 prefetch of rows/vectors (experiments; off by default)
@@ -206,6 +212,7 @@ struct Index {
                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
     idb_status narrow_points_to_bf16();                                  // d_points (f32) -> d_points_bf16, frees d_points
+    idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
     int search_grid() const;
     // Fills the visited-tier fields of `a` (pool, gslots, ...) for a traversal with this ef and returns the launch window.

@@ -93,7 +93,7 @@ __global__ void __launch_bounds__(kSearchWarps * 32, OCC) search_kernel(SearchAr
         long_q_bind<EF_T>(q, smem_raw, a.g.nchunks, warp, kSearchWarps);
         q_from_f32<CH>(q, a.queries + qi * a.g.nchunks, a.g.nchunks, lane);
 
-        descend<CH, ROW_T, EF_T, B, false, RT, FULL, TMA>(a.g, s, q, 0u, a.ef, lane, a.counters ? a.counters + qi * 4 : nullptr);
+        descend<CH, ROW_T, EF_T, B, false, RT, FULL, TMA, /*SCREEN=*/!TMA>(a.g, s, q, 0u, a.ef, lane, a.counters ? a.counters + qi * 4 : nullptr);
 
         const bool ok = s.status == kQueryOk;
         const uint64_t* near = (s.near_base + s.cur * s.near_len);
@@ -106,6 +106,7 @@ __global__ void __launch_bounds__(kSearchWarps * 32, OCC) search_kernel(SearchAr
             if (a.out_dist) a.out_dist[qi * a.k + j] = j < len ? reported_distance(key_dbits(key), a.metric) : __int_as_float(0x7f800000);
         }
         if (lane == 0) {
+            if (a.full_tally) atomicAdd(a.full_tally, (unsigned long long)s.n_full);
             if (a.out_len) a.out_len[qi] = len;
             a.status[qi] = s.status;
             if (!ok) {

@@ -24,6 +24,7 @@ SYMBOLS = [
     "idb_comm_unique_id", "idb_comm_create", "idb_comm_free", "idb_index_set_id_map", "idb_sharded_search_batch_f32",
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
+    "idb_last_search_full_fetches", "idb_debug_screen_bound",
 ]
 
 
@@ -79,6 +80,8 @@ def lib():
     L.idb_last_search_counters.argtypes = [vp, C.c_uint64, u64p]
     L.idb_last_search_failures.argtypes = [vp, C.c_uint32, u32p]
     L.idb_last_search_retried.argtypes = [vp, C.c_uint32, u32p]
+    L.idb_last_search_full_fetches.argtypes = [vp, C.c_uint32, u64p]
+    L.idb_debug_screen_bound.argtypes = [vp, f32p, C.c_uint64, u32p, C.c_uint64, f32p, f32p]
     L.idb_index_num_lanes.restype = C.c_uint32
     L.idb_index_lane_stream.argtypes = [vp, C.c_uint32]
     L.idb_index_lane_stream.restype = vp
@@ -260,6 +263,22 @@ class Index:
         out = C.c_uint32()
         check(lib().idb_last_search_retried(self._h, lane, C.byref(out)))
         return int(out.value)
+
+    def last_full_fetches(self, lane=0xFFFFFFFF):
+        """Candidate rows the last call fetched in full (all queries; equal to the summed distance counters when unscreened)."""
+        out = C.c_uint64()
+        check(lib().idb_last_search_full_fetches(self._h, lane, C.byref(out)))
+        return int(out.value)
+
+    def screen_bound(self, queries, pairs):
+        """(bound, canonical distance) per (query index, PointId) pair: the screening bound K1 compares with the furthest distance."""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        p = np.ascontiguousarray(pairs, dtype=np.uint32).reshape(-1, 2)
+        bound = np.empty(p.shape[0], dtype=np.float32)
+        dist = np.empty(p.shape[0], dtype=np.float32)
+        check(lib().idb_debug_screen_bound(self._h, ptr(q, C.c_float), q.shape[0], ptr(p, C.c_uint32), p.shape[0],
+                                           ptr(bound, C.c_float), ptr(dist, C.c_float)))
+        return bound, dist
 
     def last_failures(self, lane=0):
         out = C.c_uint32()
