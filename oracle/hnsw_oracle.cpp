@@ -706,18 +706,11 @@ ORC_API void orc_shuffle(uint64_t n, uint64_t seed, uint32_t* out_ids) {
     shuffle_ids(n, seed, order, out_ids);
 }
 
-ORC_API orc_index* orc_build(const float* rows, uint64_t n, uint32_t dim, const orc_params* p, uint32_t* out_ids) {
-    auto* ix = new orc_index();
-    ix->M = p->M;
-    ix->dim = dim;
-    ix->stride = ((size_t)dim + 3) / 4 * 4;
-    ix->n = n;
-    ix->ef_search = p->ef_search;
-    ix->metric = p->metric;
-    if (n == 0) return ix;  // core:224-234
-    if (n >= 0xFFFFFFFFull) { delete ix; return nullptr; }  // core:256
+// Shared by orc_build and orc_build_batched, for n >= 1: layer schedule (core:238-249), shuffle and shuffled rows
+// (core:257-270), an all-INVALID zero layer and empty snapshots.  Returns the (size, cumulative) pairs, top layer first.
+static std::vector<std::pair<uint64_t, uint64_t>> init_index(orc_index* ix, const float* rows, uint64_t n, uint32_t dim,
+                                                             const orc_params* p, uint32_t* out_ids) {
     const uint32_t M = p->M;
-
     auto sizes = layer_sizes(n, M, p->ml);
     const uint32_t num_layers = (uint32_t)sizes.size(), top = num_layers - 1;
     ix->layer_n.assign(num_layers, 0);
@@ -733,6 +726,33 @@ ORC_API orc_index* orc_build(const float* rows, uint64_t n, uint32_t dim, const 
 
     ix->zero.assign(n * 2 * (size_t)M, INVALID);
     ix->layers.assign(top, {});
+    return sizes;
+}
+
+// UpperNode::from_zero (types:65-71) for nodes [0, end) of a finished layer.
+static void snapshot_layer(orc_index* ix, uint32_t layer, uint64_t end, int threads) {
+    const uint32_t M = ix->M;
+    auto& snap = ix->layers[layer - 1];
+    snap.resize(end * (size_t)M);
+    parallel_for(0, end, threads, 4096, [&](uint64_t v, int) {
+        std::memcpy(snap.data() + v * M, ix->zero.data() + v * 2 * M, M * sizeof(uint32_t));
+    });
+}
+
+ORC_API orc_index* orc_build(const float* rows, uint64_t n, uint32_t dim, const orc_params* p, uint32_t* out_ids) {
+    auto* ix = new orc_index();
+    ix->M = p->M;
+    ix->dim = dim;
+    ix->stride = ((size_t)dim + 3) / 4 * 4;
+    ix->n = n;
+    ix->ef_search = p->ef_search;
+    ix->metric = p->metric;
+    if (n == 0) return ix;  // core:224-234
+    if (n >= 0xFFFFFFFFull) { delete ix; return nullptr; }  // core:256
+
+    const auto sizes = init_index(ix, rows, n, dim, p, out_ids);
+    const uint32_t num_layers = (uint32_t)sizes.size(), top = num_layers - 1;
+    const int threads = std::max(1, p->threads);
 
     Construction st;
     st.ix = ix;
@@ -753,15 +773,207 @@ ORC_API orc_index* orc_build(const float* rows, uint64_t n, uint32_t dim, const 
         } else {
             parallel_for(start, end, threads, 16, [&](uint64_t v, int) { st.insert((uint32_t)v, layer); });
         }
-        if (layer != 0) {  // UpperNode::from_zero (types:65-71)
-            auto& snap = ix->layers[layer - 1];
-            snap.resize(end * (size_t)M);
-            parallel_for(0, end, threads, 4096, [&](uint64_t v, int) {
-                std::memcpy(snap.data() + v * M, ix->zero.data() + v * 2 * M, M * sizeof(uint32_t));
-            });
-        }
+        if (layer != 0) snapshot_layer(ix, layer, end, threads);
     }
     for (auto& pr : st.pool) { delete pr.first; delete pr.second; }
+    return ix;
+}
+
+// ================================================================================================
+// Batched build: a CPU statement of THIS LIBRARY's batch schedule (DESIGN.md §6, csrc/build.cu), not of the reference.
+// The reference inserts concurrently under rayon and per-row locks, so its threaded graphs are not reproducible; the
+// library replaces that with a deterministic schedule, and this section states that schedule with the oracle's own
+// push / search_layer / select_heuristic, so batched GPU graphs can be checked bit for bit.  Per layer, top first:
+//   schedule  b = 1 on the top layer, else min(max_batch, max(1, g0 / growth)), clipped to the end of the layer;
+//   KA        every insert of a batch runs Construction::insert's descent against the zero layer as it stood when
+//             the batch began (no row changes during the batch);
+//   K2        each insert selects its own neighbours (select_heuristic, or the first min(len, 2M) in simple mode),
+//             writes its whole row and emits (target <- new) link requests;
+//   K2'       requests sorted by (target, new).  Heuristic mode: each target row is re-pruned in rounds of at most
+//             kNewCap = 32 new ids, ascending; a round's candidates are its new ids followed by the row's valid prefix,
+//             pushed in that order with ef = ef_construction (push admission, no truncation), then select_heuristic,
+//             then the whole row is rewritten.  Simple mode: one request at a time in ascending `new` order, with the
+//             reversed-comparator binary search and ZeroNode::insert of core:497-515.
+// With max_batch = 1 this is exactly orc_build's sequential order.  Inserts of a batch and targets of a batch run on
+// `threads` workers; each touches only its own output, so the graph does not depend on the thread count.
+// ================================================================================================
+struct orc_batch_stats {
+    uint64_t batches;                   // batches over all layers
+    uint64_t max_batch;                 // inserts in the largest batch
+    uint64_t link_requests;             // (target <- new) pairs, over all batches
+    uint64_t targets;                   // distinct target rows, summed over batches
+    uint64_t max_target_requests;       // most requests one target received in one batch (the largest hub)
+    uint64_t multi_new_rounds;          // heuristic re-prune rounds with more than one new id
+    uint64_t multi_round_targets;       // heuristic targets that needed more than one round in one batch
+    uint64_t admission_limited_rounds;  // heuristic rounds with ef_construction < C (push admission may reject)
+    uint64_t simple_multi_targets;      // simple-mode targets with more than one request in one batch
+    uint64_t max_insert_dist;           // most distance evaluations of one layer-0 insert on layer 0 (<= ids it visited there)
+};
+
+namespace {
+constexpr uint32_t kNewCap = 32;  // new ids per re-prune round (build_kernels.cuh)
+
+void merge_stats(orc_batch_stats& a, const orc_batch_stats& b) {
+    a.link_requests += b.link_requests;
+    a.targets += b.targets;
+    a.max_target_requests = std::max(a.max_target_requests, b.max_target_requests);
+    a.multi_new_rounds += b.multi_new_rounds;
+    a.multi_round_targets += b.multi_round_targets;
+    a.admission_limited_rounds += b.admission_limited_rounds;
+    a.simple_multi_targets += b.simple_multi_targets;
+    a.max_insert_dist = std::max(a.max_insert_dist, b.max_insert_dist);
+}
+}  // namespace
+
+// out_batches (optional): (first PointId, inserts) of the first batch_cap batches, in build order.
+// row_batch (optional, n entries): index of the last batch that wrote each zero row (INVALID: never written).
+ORC_API orc_index* orc_build_batched(const float* rows, uint64_t n, uint32_t dim, const orc_params* p, uint32_t max_batch,
+                                     uint32_t growth, orc_batch_stats* stats, uint64_t* out_batches, uint64_t batch_cap,
+                                     uint32_t* row_batch, uint32_t* out_ids) {
+    orc_batch_stats total;
+    std::memset(&total, 0, sizeof(total));
+    if (stats) *stats = total;
+    if (row_batch) std::fill(row_batch, row_batch + n, INVALID);
+    if (max_batch == 0 || growth == 0 || p->extend_candidates) return nullptr;  // the library rejects extend_candidates
+    auto* ix = new orc_index();
+    ix->M = p->M;
+    ix->dim = dim;
+    ix->stride = ((size_t)dim + 3) / 4 * 4;
+    ix->n = n;
+    ix->ef_search = p->ef_search;
+    ix->metric = p->metric;
+    if (n == 0) return ix;
+    if (n >= 0xFFFFFFFFull) { delete ix; return nullptr; }
+
+    const auto sizes = init_index(ix, rows, n, dim, p, out_ids);
+    const uint32_t num_layers = (uint32_t)sizes.size(), top = num_layers - 1;
+    const int threads = std::max(1, p->threads);
+    const uint32_t M = p->M, cap = 2 * M;
+    const size_t efc = p->ef_construction;
+    Heuristic h;
+    h.on = p->heuristic != 0;
+    h.keep_pruned = p->keep_pruned != 0;
+    const Points pts = ix->pts();
+    auto zrow = [&](uint32_t pid) { return ix->zero.data() + (size_t)pid * cap; };
+    auto no_rows = [](uint32_t, uint32_t, uint32_t*) { return 0u; };  // extend_candidates is off: no row is read
+
+    std::vector<Search> searches(threads);
+    for (auto& s : searches) s.visited.with_capacity(n);
+    std::vector<orc_batch_stats> tstats(threads);
+    std::vector<uint32_t> found;   // max_batch x 2M: own rows of the batch's inserts
+    std::vector<uint64_t> pairs;   // (target << 32 | new)
+    std::vector<uint64_t> seg;     // start index of each target's requests in `pairs`
+    uint64_t batch_index = 0;
+
+    for (uint32_t li = 0; li < num_layers; ++li) {
+        const uint32_t layer = num_layers - li - 1;
+        const uint64_t size = sizes[li].first, cumulative = sizes[li].second;
+        const uint64_t start = std::max<uint64_t>(cumulative - size, 1), end = cumulative;
+        const uint32_t num = layer == 0 ? 2 * M : M;  // core:445
+        for (uint64_t g0 = start; g0 < end;) {
+            uint64_t b = 1;
+            if (layer != top) b = std::min<uint64_t>(max_batch, std::max<uint64_t>(1, g0 / growth));
+            b = std::min<uint64_t>(b, end - g0);
+            if (out_batches && batch_index < batch_cap) { out_batches[2 * batch_index] = g0; out_batches[2 * batch_index + 1] = b; }
+            total.batches++;
+            total.max_batch = std::max<uint64_t>(total.max_batch, b);
+            for (auto& t : tstats) std::memset(&t, 0, sizeof(t));
+
+            // ---- KA + K2: every insert against the zero layer as the batch found it ----
+            found.assign(b * cap, INVALID);
+            parallel_for(0, b, threads, 4, [&](uint64_t w, int t) {
+                const uint32_t neu = (uint32_t)(g0 + w);
+                const float* point = pts.row(neu);
+                Search& s = searches[t];
+                s.reset();
+                push(s, 0, point, pts);  // core:444
+                for (uint32_t cur = top;; --cur) {  // core:447-463
+                    s.ef = cur <= layer ? efc : 1;
+                    if (cur > layer) {
+                        const uint32_t* snap = ix->layers[cur - 1].data();
+                        search_layer(s, point, [&](uint32_t pid, uint32_t links, uint32_t* buf) {
+                            return copy_row(snap + (size_t)pid * M, M, links, buf); }, pts, num);
+                        s.cull();
+                    } else {
+                        s.n_dist = 0;
+                        search_layer(s, point, [&](uint32_t pid, uint32_t links, uint32_t* buf) {
+                            return copy_row(zrow(pid), cap, links, buf); }, pts, num);
+                        if (layer == 0) tstats[t].max_insert_dist = std::max<uint64_t>(tstats[t].max_insert_dist, s.n_dist);
+                        break;
+                    }
+                    if (cur == 0) break;
+                }
+                if (h.on) select_heuristic(s, point, no_rows, pts, M, h);  // core:470-472
+                else if (s.nearest.size() > cap) s.nearest.resize(cap);  // core:466-469
+                for (size_t i = 0; i < s.nearest.size(); ++i) found[w * cap + i] = key_pid(s.nearest[i]);
+            });
+
+            // ---- own rows and link requests, grouped by target ----
+            pairs.clear();
+            for (uint64_t w = 0; w < b; ++w) {
+                const uint32_t neu = (uint32_t)(g0 + w);
+                std::memcpy(zrow(neu), &found[w * cap], cap * sizeof(uint32_t));
+                if (row_batch) row_batch[neu] = (uint32_t)batch_index;
+                for (uint32_t i = 0; i < cap && found[w * cap + i] != INVALID; ++i)
+                    pairs.push_back(((uint64_t)found[w * cap + i] << 32) | neu);
+            }
+            std::sort(pairs.begin(), pairs.end());
+            seg.clear();
+            for (size_t i = 0; i < pairs.size(); ++i)
+                if (i == 0 || (pairs[i] >> 32) != (pairs[i - 1] >> 32)) seg.push_back(i);
+            total.link_requests += pairs.size();
+            total.targets += seg.size();
+
+            // ---- K2': every target row, once per batch ----
+            parallel_for(0, seg.size(), threads, 16, [&](uint64_t si, int t) {
+                const size_t s0 = seg[si], s1 = si + 1 < seg.size() ? seg[si + 1] : pairs.size();
+                const uint32_t tgt = (uint32_t)(pairs[s0] >> 32);
+                const float* tpoint = pts.row(tgt);
+                uint32_t* row = zrow(tgt);
+                orc_batch_stats& ts = tstats[t];
+                ts.max_target_requests = std::max<uint64_t>(ts.max_target_requests, s1 - s0);
+                if (row_batch) row_batch[tgt] = (uint32_t)batch_index;
+                if (!h.on) {
+                    if (s1 - s0 > 1) ts.simple_multi_targets++;
+                    for (size_t r = s0; r < s1; ++r) {  // core:497-515, ascending `new`
+                        const uint32_t neu = (uint32_t)pairs[r];
+                        const uint32_t dnew = canon_bits(pts.distance(tpoint, pts.row(neu)));
+                        const size_t idx = rust_binary_search_by(cap, [&](size_t k) -> int {
+                            const uint32_t third = row[k];
+                            if (third == INVALID) return +1;
+                            const uint32_t dt = canon_bits(pts.distance(tpoint, pts.row(third)));
+                            return dnew < dt ? -1 : (dnew > dt ? +1 : 0);
+                        });
+                        if (idx < cap) {  // ZeroNode::insert (types:100-113)
+                            if (row[idx] != INVALID) std::memmove(row + idx + 1, row + idx, (cap - 1 - idx) * sizeof(uint32_t));
+                            row[idx] = neu;
+                        }
+                    }
+                    return;
+                }
+                if (s1 - s0 > kNewCap) ts.multi_round_targets++;
+                Search& s = searches[t];
+                uint32_t buf[256];
+                for (size_t r0 = s0; r0 < s1; r0 += kNewCap) {
+                    const size_t r1 = std::min<size_t>(s1, r0 + kNewCap);
+                    if (r1 - r0 > 1) ts.multi_new_rounds++;
+                    s.reset();
+                    s.ef = efc;
+                    for (size_t r = r0; r < r1; ++r) push(s, (uint32_t)pairs[r], tpoint, pts);  // the new ids first (core:626)
+                    const uint32_t cnt = copy_row(row, cap, cap, buf);
+                    for (uint32_t j = 0; j < cnt; ++j) push(s, buf[j], tpoint, pts);  // then the row (core:627-629)
+                    if (efc < (r1 - r0) + cnt) ts.admission_limited_rounds++;
+                    select_heuristic(s, tpoint, no_rows, pts, M, h);
+                    for (uint32_t i = 0; i < cap; ++i) row[i] = i < s.nearest.size() ? key_pid(s.nearest[i]) : INVALID;
+                }
+            });
+            for (const auto& t : tstats) merge_stats(total, t);
+            g0 += b;
+            batch_index++;
+        }
+        if (layer != 0) snapshot_layer(ix, layer, end, threads);
+    }
+    if (stats) *stats = total;
     return ix;
 }
 

@@ -28,6 +28,12 @@ class Params(C.Structure):
     ]
 
 
+class BatchStats(C.Structure):
+    _fields_ = [(name, C.c_uint64) for name in (
+        "batches", "max_batch", "link_requests", "targets", "max_target_requests", "multi_new_rounds", "multi_round_targets",
+        "admission_limited_rounds", "simple_multi_targets", "max_insert_dist")]
+
+
 def build_lib(force=False):
     if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(os.path.join(_HERE, "hnsw_oracle.cpp")):
         subprocess.check_call(["make", "-C", _HERE, "-s"])
@@ -62,6 +68,9 @@ def lib():
     L.orc_rng_kat.restype = None
     L.orc_build.restype = C.c_void_p
     L.orc_build.argtypes = [f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), u32p]
+    L.orc_build_batched.restype = C.c_void_p
+    L.orc_build_batched.argtypes = [f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), C.c_uint32, C.c_uint32, C.POINTER(BatchStats),
+                                    u64p, C.c_uint64, u32p, u32p]
     L.orc_from_graph.restype = C.c_void_p
     L.orc_from_graph.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_uint32,
                                  C.POINTER(u32p), u64p, C.c_int32]
@@ -226,6 +235,31 @@ def build(rows, **kw):
     if not h:
         raise ValueError("orc_build failed (N >= u32::MAX?)")
     return Index(h), ids
+
+
+def build_batched(rows, max_batch, growth, threads=1, **kw):
+    """The library's batched build schedule (DESIGN.md §6), stated on the CPU.  Returns (Index, ids, stats).
+
+    max_batch / growth: the schedule's cap and divisor (the library takes them from insert_batch, or from IDB_BUILD_MAXBATCH /
+    IDB_BUILD_GROWTH when insert_batch is 0; its defaults are 16384 and 8).  stats: the BatchStats counters as a dict, plus
+    "bounds" (batches x 2: first PointId, inserts, in build order) and "row_batch" (per zero row, the last batch that wrote it).
+    """
+    rows = _f32(rows)
+    n, dim = rows.shape
+    p = default_params(threads=threads, **kw)
+    ids = np.empty(n, dtype=np.uint32)
+    st = BatchStats()
+    cap = n + 1  # a batch holds at least one insert
+    bounds = np.zeros((cap, 2), dtype=np.uint64)
+    row_batch = np.empty(n, dtype=np.uint32)
+    h = lib().orc_build_batched(_p(rows, C.c_float), n, dim, C.byref(p), max_batch, growth, C.byref(st), _p(bounds, C.c_uint64), cap,
+                                _p(row_batch, C.c_uint32), _p(ids, C.c_uint32))
+    if not h:
+        raise ValueError("orc_build_batched failed (max_batch or growth 0, extend_candidates, or N >= u32::MAX)")
+    stats = {name: int(getattr(st, name)) for name, _ in BatchStats._fields_}
+    stats["bounds"] = bounds[:stats["batches"]].copy()
+    stats["row_batch"] = row_batch
+    return Index(h), ids, stats
 
 
 def from_graph(g, metric=0):
