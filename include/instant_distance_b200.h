@@ -163,6 +163,11 @@ IDB_API idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint
  * already proves they would not be admitted are not fetched, so it is smaller.  Results are the same either way.
  * lane = 0xFFFFFFFF: the lane the last call on this index used. */
 IDB_API idb_status idb_last_search_full_fetches(idb_index* index, uint32_t lane, uint64_t* out_rows);
+/* Diagnostics: which instantiation of the search kernel the last call on `lane` launched (its main pass; the retry pass uses the same
+ * one).  out (8 u32) = {CH (float4 chunks per lane of a row, 0 = the long-row kernel), ROW_T, EF_T, B (rows in flight per lane), 1 if the
+ * rows are bf16, 1 if FULL (no chunk predicates), 1 if TMA, the IDB_VARIANT case taken (0 = the default dispatch)}; all zeros when
+ * the last call launched no kernel.  lane = 0xFFFFFFFF: the lane the last call on this index used. */
+IDB_API idb_status idb_last_search_kernel(idb_index* index, uint32_t lane, uint32_t* out);
 /* enabled = 1: reserve persisting L2 for the visited tables on `device` (see idb_search_batch_f32).  enabled = 0 (the default):
  * this library never touches the device's persisting-L2 limit nor attaches access-policy windows on `device`. */
 IDB_API idb_status idb_device_set_persisting_l2(int32_t device, int32_t enabled);

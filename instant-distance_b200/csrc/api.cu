@@ -528,6 +528,8 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     a.out_keys = out_keys;
     a.id_map = d_id_map;
     a.full_tally = reinterpret_cast<unsigned long long*>(ln.ctrl + 8);  // K1 and the retry pass both add to it
+    std::memset(ln.last_kernel, 0, sizeof(ln.last_kernel));
+    a.launched = ln.last_kernel;
 
     const int ch = (int)((nchunks + 31) / 32);
     if (ch > 8 && (nchunks + 31) / 32 * 512 > 40 * 1024)
@@ -560,6 +562,7 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     r.work_counter = reinterpret_cast<unsigned long long*>(ln.ctrl + 32);
     r.fail_count = reinterpret_cast<uint32_t*>(ln.ctrl + 48);
     r.fail_list = nullptr;       // failures of the retry pass are only counted (and visible in status[])
+    r.launched = nullptr;        // same instantiation as K1; last_kernel describes the main launch
     r.pool = ctx->retry_pool();
     r.gslots = kRetrySlots;
     r.gshift = 32 - 18;
@@ -973,6 +976,18 @@ idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint32_t* ou
     CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
     CUDA_TRY(cudaStreamSynchronize(ln.stream));
     *out_retried = ctrl[4];
+    return IDB_OK;
+}
+
+idb_status idb_last_search_kernel(idb_index* index, uint32_t lane, uint32_t* out) {
+    if (!index || !out) return fail(IDB_ERR_INVALID_ARG, "null argument");
+    Index* ix = reinterpret_cast<Index*>(index);
+    if (lane == 0xFFFFFFFFu) lane = (uint32_t)ix->last_lane.load();
+    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
+    Lane& ln = ix->lanes[lane];
+    std::lock_guard<std::mutex> lk(ln.mu);
+    std::memset(out, 0, 8 * sizeof(uint32_t));
+    if (ln.last_nq != 0) std::memcpy(out, ln.last_kernel, sizeof(ln.last_kernel));
     return IDB_OK;
 }
 

@@ -62,6 +62,7 @@ struct SearchArgs {
     int variant;                       // tuning variant of the kernel template (0 = default)
     uint32_t metric;                   // Metric: how out_dist reports a key's distance (out_keys always carry the key's own bits)
     unsigned long long* full_tally;    // optional: += rows fetched in full (the rows the screen did not drop), over the call
+    uint32_t* launched;                // HOST memory, optional: launch_search writes the K1 instantiation it launched (Lane::last_kernel)
 };
 
 // Persisting-L2 access-policy window attached to a launch (the b16 visited tables), or none.
@@ -143,6 +144,8 @@ struct Lane {
     uint64_t ctrl_nq = 0;
     uint64_t last_nq = 0;
     uint32_t last_launches = 0;
+    // the template arguments of the lane's last main K1 launch: {CH, ROW_T, EF_T, B, bf16 rows, FULL, TMA, IDB_VARIANT taken}
+    uint32_t last_kernel[8] = {};
     void free_all();
 };
 

@@ -2,18 +2,19 @@
 #include "search_kernel.cuh"
 namespace idb {
 cudaError_t dispatch_search_ch1(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    // tuning variants of the headline shape (ROW_T=2, EF_T=4): rows in flight per lane x resident CTAs per SM
-    if (a.variant && row_t <= 2 && ef_t <= 4) {
+    // tuning variants of the headline shape (ROW_T=2, EF_T=4): rows in flight per lane x resident CTAs per SM.  They are
+    // instantiated for f32 rows only: a bf16 index takes the default dispatch below.
+    if (a.variant && !a.g.bf16 && row_t <= 2 && ef_t <= 4) {
         switch (a.variant) {
-            case 1: return launch_search<1, 2, 4, 8, occ_for_warps(20)>(a, grid, st, win);
-            case 2: return launch_search<1, 2, 4, 8, occ_for_warps(24)>(a, grid, st, win);
-            case 3: return launch_search<1, 2, 4, 4, occ_for_warps(32)>(a, grid, st, win);
-            case 4: return launch_search<1, 2, 4, 16, occ_for_warps(12)>(a, grid, st, win);
+            case 1: return launch_search<1, 2, 4, 8, occ_for_warps(20)>(a, grid, st, win, 1);
+            case 2: return launch_search<1, 2, 4, 8, occ_for_warps(24)>(a, grid, st, win, 2);
+            case 3: return launch_search<1, 2, 4, 4, occ_for_warps(32)>(a, grid, st, win, 3);
+            case 4: return launch_search<1, 2, 4, 16, occ_for_warps(12)>(a, grid, st, win, 4);
             // EXPERIMENT: rows via cp.async.bulk into a shared-memory ring, no register staging
-            case 5: if (!a.g.bf16) return launch_search<1, 2, 4, 16, occ_for_warps(16), RowF32, false, true>(a, grid, st, win); break;
-            case 6: if (!a.g.bf16) return launch_search<1, 2, 4, 8, occ_for_warps(20), RowF32, false, true>(a, grid, st, win); break;
-            case 7: if (!a.g.bf16) return launch_search<1, 2, 4, 8, occ_for_warps(24), RowF32, false, true>(a, grid, st, win); break;
-            case 8: if (!a.g.bf16) return launch_search<1, 2, 4, 32, occ_for_warps(8), RowF32, false, true>(a, grid, st, win); break;
+            case 5: return launch_search<1, 2, 4, 16, occ_for_warps(16), RowF32, false, true>(a, grid, st, win, 5);
+            case 6: return launch_search<1, 2, 4, 8, occ_for_warps(20), RowF32, false, true>(a, grid, st, win, 6);
+            case 7: return launch_search<1, 2, 4, 8, occ_for_warps(24), RowF32, false, true>(a, grid, st, win, 7);
+            case 8: return launch_search<1, 2, 4, 32, occ_for_warps(8), RowF32, false, true>(a, grid, st, win, 8);
             default: break;
         }
     }

@@ -2,6 +2,7 @@
 // Instantiated once per CH (float4 chunks per lane) in search_chN.cu so the translation units build in parallel.
 #pragma once
 #include <cstring>
+#include <type_traits>
 
 #include "internal.cuh"
 
@@ -142,14 +143,21 @@ static cudaError_t launch_with_window(Kern kern, int grid, int block, int smem, 
     return cudaLaunchKernelEx(&cfg, kern, a);
 }
 
+// variant: the IDB_VARIANT case that chose this instantiation (0 = the default dispatch); recorded with the template arguments.
 template <int CH, int ROW_T, int EF_T, int B, int OCC = kSearchCtasPerSm, class RT = RowF32, bool FULL = false, bool TMA = false>
-static cudaError_t launch_search(const SearchArgs& a, int grid, cudaStream_t stream, const LaunchWindow& win) {
+static cudaError_t launch_search(const SearchArgs& a, int grid, cudaStream_t stream, const LaunchWindow& win, int variant = 0) {
     const int smem = (WarpSmem<EF_T>::kBytes + (CH == 0 ? (int)long_q_bytes(a.g.nchunks) : 0)) * kSearchWarps +
                      (TMA ? 64 + kSearchWarps * B * (int)a.g.nchunks * 16 : 0);
     auto kern = search_kernel<CH, ROW_T, EF_T, B, OCC, RT, FULL, TMA>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
-    return launch_with_window(kern, grid, kSearchWarps * 32, smem, stream, win, a);
+    e = launch_with_window(kern, grid, kSearchWarps * 32, smem, stream, win, a);
+    if (e == cudaSuccess && a.launched) {
+        const uint32_t cell[8] = {CH, ROW_T, EF_T, B, std::is_same<RT, RowBF16>::value ? 1u : 0u, FULL ? 1u : 0u, TMA ? 1u : 0u,
+                                  (uint32_t)variant};
+        std::memcpy(a.launched, cell, sizeof(cell));
+    }
+    return e;
 }
 
 template <int CH, int ROW_T, int EF_T, int B, class RT>

@@ -24,7 +24,7 @@ SYMBOLS = [
     "idb_comm_unique_id", "idb_comm_create", "idb_comm_free", "idb_index_set_id_map", "idb_sharded_search_batch_f32",
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
-    "idb_last_search_full_fetches", "idb_debug_screen_bound",
+    "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel",
 ]
 
 
@@ -82,6 +82,7 @@ def lib():
     L.idb_last_search_retried.argtypes = [vp, C.c_uint32, u32p]
     L.idb_last_search_full_fetches.argtypes = [vp, C.c_uint32, u64p]
     L.idb_debug_screen_bound.argtypes = [vp, f32p, C.c_uint64, u32p, C.c_uint64, f32p, f32p]
+    L.idb_last_search_kernel.argtypes = [vp, C.c_uint32, u32p]
     L.idb_index_num_lanes.restype = C.c_uint32
     L.idb_index_lane_stream.argtypes = [vp, C.c_uint32]
     L.idb_index_lane_stream.restype = vp
@@ -269,6 +270,14 @@ class Index:
         out = C.c_uint64()
         check(lib().idb_last_search_full_fetches(self._h, lane, C.byref(out)))
         return int(out.value)
+
+    KERNEL_FIELDS = ("ch", "row_t", "ef_t", "b", "bf16", "full", "tma", "variant")
+
+    def last_kernel(self, lane=0xFFFFFFFF):
+        """The search-kernel instantiation the last call launched, as a dict over KERNEL_FIELDS (all zeros: none launched)."""
+        out = (C.c_uint32 * 8)()
+        check(lib().idb_last_search_kernel(self._h, lane, out))
+        return dict(zip(self.KERNEL_FIELDS, (int(v) for v in out)))
 
     def screen_bound(self, queries, pairs):
         """(bound, canonical distance) per (query index, PointId) pair: the screening bound K1 compares with the furthest distance."""
