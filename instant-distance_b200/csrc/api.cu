@@ -35,14 +35,14 @@ cudaError_t dispatch_search_ch6(const SearchArgs&, int, int, int, cudaStream_t, 
 cudaError_t dispatch_search_ch8(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
 cudaError_t dispatch_search_long(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
 
-cudaError_t dispatch_search(const SearchArgs& a, int ch, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    switch (ch) {
+static cudaError_t dispatch_search(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
+    switch (kernel_ch(a.g.nchunks)) {
         case 1: return dispatch_search_ch1(a, row_t, ef_t, grid, st, win);
         case 2: return dispatch_search_ch2(a, row_t, ef_t, grid, st, win);
         case 3: return dispatch_search_ch3(a, row_t, ef_t, grid, st, win);
         case 4: return dispatch_search_ch4(a, row_t, ef_t, grid, st, win);
-        case 5: case 6: return dispatch_search_ch6(a, row_t, ef_t, grid, st, win);
-        case 7: case 8: return dispatch_search_ch8(a, row_t, ef_t, grid, st, win);
+        case 6: return dispatch_search_ch6(a, row_t, ef_t, grid, st, win);
+        case 8: return dispatch_search_ch8(a, row_t, ef_t, grid, st, win);
         default: return dispatch_search_long(a, row_t, ef_t, grid, st, win);
     }
 }
@@ -189,19 +189,23 @@ TablePool DeviceCtx::main_pool(bool b16) const {
     tp.tie_cap = kTieCap;
     return tp;
 }
-TablePool DeviceCtx::retry_pool() const {
-    TablePool tp;
-    tp.slot_masks = slot_masks;
-    tp.fixed_word = sm_ids;
-    tp.word_base = (uint32_t)sm_ids;
-    tp.slots_per_word = kRetryCtas;
-    tp.vis_tables = retry_tables;
-    tp.vis_stride = kRetrySlots;
-    tp.vis_ext = nullptr;
-    tp.ext_stride = 0;
-    tp.tie_tables = retry_ties;
-    tp.tie_cap = kRetryTieCap;
-    return tp;
+VisTier DeviceCtx::retry_tier() const {
+    VisTier t = {};
+    t.pool.slot_masks = slot_masks;
+    t.pool.fixed_word = sm_ids;
+    t.pool.word_base = (uint32_t)sm_ids;
+    t.pool.slots_per_word = kRetryCtas;
+    t.pool.vis_tables = retry_tables;
+    t.pool.vis_stride = kRetrySlots;
+    t.pool.vis_ext = nullptr;
+    t.pool.ext_stride = 0;
+    t.pool.tie_tables = retry_ties;
+    t.pool.tie_cap = kRetryTieCap;
+    t.gslots = kRetrySlots;
+    t.gshift = 32 - 18;
+    static_assert(kRetrySlots == 1u << 18, "gshift above");
+    t.mode = kVisHash;
+    return t;
 }
 
 idb_status DeviceCtx::acquire(int device, DeviceCtx** out) {
@@ -392,6 +396,23 @@ Lane& Index::pick_lane() {
     return ln;
 }
 
+idb_status Index::last_search(uint32_t lane, bool latest, SearchCtrl* ctrl, uint32_t* kernel) {
+    if (latest && lane == 0xFFFFFFFFu) lane = (uint32_t)last_lane.load();
+    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
+    Lane& ln = lanes[lane];
+    std::lock_guard<std::mutex> lk(ln.mu);
+    if (ctrl) *ctrl = SearchCtrl();
+    if (kernel) std::memset(kernel, 0, sizeof(ln.last_kernel));
+    if (ln.last_nq == 0) return IDB_OK;
+    if (kernel) std::memcpy(kernel, ln.last_kernel, sizeof(ln.last_kernel));
+    if (ctrl) {
+        CUDA_TRY(cudaSetDevice(device));
+        CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
+        CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    }
+    return IDB_OK;
+}
+
 idb_status Index::attach_window(Lane& ln, const LaunchWindow& win) {
     if (ln.win_base == win.base && ln.win_bytes == win.bytes) return IDB_OK;
     cudaStreamAttrValue av;
@@ -411,12 +432,12 @@ idb_status Index::attach_window(Lane& ln, const LaunchWindow& win) {
 
 idb_status Index::ensure_lane_scratch(Lane& ln, uint64_t nq) {
     if (!ln.ctrl) {
-        CUDA_TRY(cudaMalloc(&ln.ctrl, 64));
-        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&ln.h_ctrl), 128, cudaHostAllocDefault));  // [0,16): sampled tally, [16,32): host API
+        CUDA_TRY(cudaMalloc(&ln.ctrl, sizeof(SearchCtrl)));
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&ln.h_ctrl), 2 * sizeof(SearchCtrl), cudaHostAllocDefault));
         CUDA_TRY(cudaEventCreateWithFlags(&ln.ev_ctrl, cudaEventDisableTiming));
     }
     if (ln.ctrl_pending && cudaEventQuery(ln.ev_ctrl) == cudaSuccess) {  // the previous call's tally has arrived
-        note_overflows(ln.ctrl_ef, ln.ctrl_nq, ln.h_ctrl[4], ln.ctrl_b16);
+        note_overflows(ln.ctrl_ef, ln.ctrl_nq, ln.h_ctrl[0].main.fail_count, ln.ctrl_b16);
         ln.ctrl_pending = false;
     }
     CUDA_TRY(ensure(ln.status, ln.status_cap, nq));
@@ -433,7 +454,7 @@ idb_status Index::ensure_lane_scratch(Lane& ln, uint64_t nq) {
 //   b16 (default): exact while ceil(n / 32768) <= buckets and no adjacency row repeats an id; ~2 u16 slots per id the traversal can
 //     possibly visit (2M per expansion, ~ef expansions), clamped to the per-warp stride (= what fits the persisting part of L2);
 //   else bitmap (n bits per warp) when that is no bigger than 2x the hash table, else the hash set.
-idb_status Index::select_visited_tier(uint32_t ef, SearchArgs& a, LaunchWindow& win) {
+idb_status Index::select_visited_tier(uint32_t ef, VisTier& t, LaunchWindow& win) {
     DeviceCtx& c = *ctx;
     const uint32_t efx = std::max<uint32_t>(ef, 16u);
     // 2.5 u16 slots per id the traversal can possibly insert (2M per expansion, ~ef expansions): typical load 1/3, queries handed to the
@@ -466,13 +487,13 @@ idb_status Index::select_visited_tier(uint32_t ef, SearchArgs& a, LaunchWindow& 
     if (tier < 0) tier = (b16_exact && level > 0) ? 2 : -1;
     b16_level = tier == 2 ? (level > 0 ? level : 1) : 0;
     win = LaunchWindow();
+    t = VisTier();
     if (tier == 2) {
-        a.pool = c.main_pool(true);
-        a.gslots = nb_lo * 8 + kB16Stash;
-        a.b16_nb = nb;
-        a.gshift = 0;
-        a.vis_mode = kVisB16;
-        a.b16_cap_ids = nb * b16_cap_16ths;  // <= 11 of 16 slots on average; fuller tables hand the query to the retry pass
+        t.pool = c.main_pool(true);
+        t.gslots = nb_lo * 8 + kB16Stash;
+        t.b16_nb = nb;
+        t.mode = kVisB16;
+        t.b16_cap_ids = nb * b16_cap_16ths;  // <= 11 of 16 slots on average; fuller tables hand the query to the retry pass
         idb_status st = c.reserve_l2((size_t)c.n_tables_live * std::min(b16_bytes, seg));
         if (st != IDB_OK) return st;
         if (c.l2_reserved) {
@@ -488,12 +509,10 @@ idb_status Index::select_visited_tier(uint32_t ef, SearchArgs& a, LaunchWindow& 
     const bool bitmap = tier == 1 || (tier < 0 && !vis_slots_override && (n + 31) / 32 <= 2ull * want_slots);
     idb_status st = c.ensure_big(std::max(want_slots, bitmap ? bm_words : 0u));
     if (st != IDB_OK) return st;
-    a.pool = c.main_pool(false);
-    a.gslots = bitmap ? bm_words : want_slots;
-    a.gshift = 32 - (uint32_t)std::log2((double)want_slots);
-    a.vis_mode = bitmap ? kVisBitmap : kVisHash;
-    a.b16_cap_ids = 0;
-    a.b16_nb = 0;
+    t.pool = c.main_pool(false);
+    t.gslots = bitmap ? bm_words : want_slots;
+    t.gshift = 32 - (uint32_t)std::log2((double)want_slots);
+    t.mode = bitmap ? kVisBitmap : kVisHash;
     return IDB_OK;
 }
 
@@ -506,33 +525,32 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     if (ef > 1024) return fail(IDB_ERR_UNSUPPORTED, "ef_search %u > 1024 (on an index of more than 1024 points) is not supported", ef);
     idb_status st = ensure_lane_scratch(ln, nq);
     if (st != IDB_OK) return st;
-    CUDA_TRY(cudaMemsetAsync(ln.ctrl, 0, 64, ln.stream));
+    CUDA_TRY(cudaMemsetAsync(ln.ctrl, 0, sizeof(SearchCtrl), ln.stream));
 
     SearchArgs a;
     std::memset(&a, 0, sizeof(a));
     a.g = view();
     a.queries = reinterpret_cast<const float4*>(d_queries);
     a.metric = metric;
-    a.n_work = nq;
+    a.work.n_work = nq;
+    a.work.work_counter = &ln.ctrl->main.work_counter;
+    a.work.status = ln.status;
+    a.work.fail_count = &ln.ctrl->main.fail_count;
+    a.work.fail_list = ln.fail_list;
     a.ef = ef;
     a.k = k;
     a.out_ids = d_ids;
     a.out_dist = d_dist;
     a.out_len = d_len;
     a.counters = ln.counters;
-    a.status = ln.status;
-    a.work_counter = reinterpret_cast<unsigned long long*>(ln.ctrl);
-    a.fail_count = reinterpret_cast<uint32_t*>(ln.ctrl + 16);
-    a.fail_list = ln.fail_list;
     a.variant = variant;
     a.out_keys = out_keys;
     a.id_map = d_id_map;
-    a.full_tally = reinterpret_cast<unsigned long long*>(ln.ctrl + 8);  // K1 and the retry pass both add to it
+    a.full_tally = &ln.ctrl->full_fetches;  // K1 and the retry pass both add to it
     std::memset(ln.last_kernel, 0, sizeof(ln.last_kernel));
     a.launched = ln.last_kernel;
 
-    const int ch = (int)((nchunks + 31) / 32);
-    if (ch > 8 && (nchunks + 31) / 32 * 512 > 40 * 1024)
+    if ((nchunks + 31) / 32 * 512 > 40 * 1024)
         return fail(IDB_ERR_UNSUPPORTED, "dim %u > 10240 is not supported (the query of a long-row traversal lives in shared memory)", dim);
     const int row_t = (int)((2 * M + 31) / 32);
     const int ef_t = (int)((ef + 31) / 32);
@@ -545,33 +563,20 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
 
     std::lock_guard<std::mutex> lk(ctx->mu);  // the tables this launch uses must not be regrown under it
     LaunchWindow win;
-    st = select_visited_tier(ef, a, win);
+    st = select_visited_tier(ef, a.tier, win);
     if (st == IDB_OK) st = attach_window(ln, win);
     if (st != IDB_OK) return st;
     if (profiling) CUDA_TRY(cudaEventRecord(ln.ev0, ln.stream));
-    CUDA_TRY(dispatch_search(a, ch, row_t, ef_t, grid, ln.stream, win));
+    CUDA_TRY(dispatch_search(a, row_t, ef_t, grid, ln.stream, win));
     if (profiling) CUDA_TRY(cudaEventRecord(ln.ev1, ln.stream));
     ln.last_launches = metric == kMetricCosine ? 3 : 2;  // (the query normalisation) + K1 + the (normally idle) retry pass
 
-    // Retry pass (device-side, unconditional, normally a no-op): queries whose visited table overflowed are re-run
-    // by a few warps with 2^18-slot hash sets.  n_work is read from fail_count on the device.
-    SearchArgs r = a;
-    r.work_list = ln.fail_list;
-    r.n_work_dev = a.fail_count;
-    r.n_work = 0;
-    r.work_counter = reinterpret_cast<unsigned long long*>(ln.ctrl + 32);
-    r.fail_count = reinterpret_cast<uint32_t*>(ln.ctrl + 48);
-    r.fail_list = nullptr;       // failures of the retry pass are only counted (and visible in status[])
-    r.launched = nullptr;        // same instantiation as K1; last_kernel describes the main launch
-    r.pool = ctx->retry_pool();
-    r.gslots = kRetrySlots;
-    r.gshift = 32 - 18;
-    r.vis_mode = kVisHash;
-    static_assert(kRetrySlots == 1u << 18, "gshift above");
-    CUDA_TRY(dispatch_search(r, ch, row_t, ef_t, kRetryCtas, ln.stream, LaunchWindow()));
-    ln.last_b16 = a.vis_mode == kVisB16 ? b16_level : 0;
+    SearchArgs r = retry_pass(a, *ctx, &ln.ctrl->retry);
+    r.launched = nullptr;  // same instantiation as K1; last_kernel describes the main launch
+    CUDA_TRY(dispatch_search(r, row_t, ef_t, kRetryCtas, ln.stream, LaunchWindow()));
+    ln.last_b16 = a.tier.mode == kVisB16 ? b16_level : 0;
     if (!ln.ctrl_pending) {  // sample this call's overflow tally (one read-back in flight per lane; evaluated by a later call)
-        CUDA_TRY(cudaMemcpyAsync(ln.h_ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
+        CUDA_TRY(cudaMemcpyAsync(ln.h_ctrl, ln.ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
         CUDA_TRY(cudaEventRecord(ln.ev_ctrl, ln.stream));
         ln.ctrl_pending = true;
         ln.ctrl_b16 = ln.last_b16;
@@ -935,60 +940,36 @@ idb_status idb_search_batch_f32(idb_index* index, const float* queries, uint64_t
     // The control block comes back through PINNED memory: a device-to-pageable cudaMemcpyAsync blocks inside the driver until the
     // copy has run (i.e. until this call's K1 has finished) and stalls the launches of other caller threads meanwhile, so concurrent
     // callers would never have a second batch queued behind the running one.
-    uint32_t* ctrl = ln.h_ctrl + 16;
-    CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
+    const SearchCtrl& ctrl = ln.h_ctrl[1];
+    CUDA_TRY(cudaMemcpyAsync(ln.h_ctrl + 1, ln.ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
     CUDA_TRY(cudaStreamSynchronize(ln.stream));
     ho.finish();
-    ix->note_overflows(ef, nq, ctrl[4], ln.last_b16);
-    if (ctrl[12] != 0)  // failures that survived the retry pass
+    ix->note_overflows(ef, nq, ctrl.main.fail_count, ln.last_b16);
+    if (ctrl.retry.fail_count != 0)  // failures that survived the retry pass
         return fail(IDB_ERR_CAPACITY, "%u of %llu queries overflowed an internal per-query structure (visited table / tie list)",
-                    ctrl[12], (unsigned long long)nq);
+                    ctrl.retry.fail_count, (unsigned long long)nq);
     return IDB_OK;
 }
 
 idb_status idb_last_search_failures(idb_index* index, uint32_t lane, uint32_t* out_failed) {
     if (!index || !out_failed) return fail(IDB_ERR_INVALID_ARG, "null argument");
-    Index* ix = reinterpret_cast<Index*>(index);
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
-    Lane& ln = ix->lanes[lane];
-    std::lock_guard<std::mutex> lk(ln.mu);
-    *out_failed = 0;
-    if (!ln.ctrl || ln.last_nq == 0) return IDB_OK;
-    CUDA_TRY(cudaSetDevice(ix->device));
-    uint32_t ctrl[16];
-    CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    *out_failed = ctrl[12];
-    return IDB_OK;
+    SearchCtrl c;
+    idb_status st = reinterpret_cast<Index*>(index)->last_search(lane, false, &c, nullptr);
+    if (st == IDB_OK) *out_failed = c.retry.fail_count;
+    return st;
 }
 
 idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint32_t* out_retried) {
     if (!index || !out_retried) return fail(IDB_ERR_INVALID_ARG, "null argument");
-    Index* ix = reinterpret_cast<Index*>(index);
-    if (lane == 0xFFFFFFFFu) lane = (uint32_t)ix->last_lane.load();  // the lane of the last call issued on this index
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
-    Lane& ln = ix->lanes[lane];
-    std::lock_guard<std::mutex> lk(ln.mu);
-    *out_retried = 0;
-    if (!ln.ctrl || ln.last_nq == 0) return IDB_OK;
-    CUDA_TRY(cudaSetDevice(ix->device));
-    uint32_t ctrl[16];
-    CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    *out_retried = ctrl[4];
-    return IDB_OK;
+    SearchCtrl c;
+    idb_status st = reinterpret_cast<Index*>(index)->last_search(lane, true, &c, nullptr);
+    if (st == IDB_OK) *out_retried = c.main.fail_count;
+    return st;
 }
 
 idb_status idb_last_search_kernel(idb_index* index, uint32_t lane, uint32_t* out) {
     if (!index || !out) return fail(IDB_ERR_INVALID_ARG, "null argument");
-    Index* ix = reinterpret_cast<Index*>(index);
-    if (lane == 0xFFFFFFFFu) lane = (uint32_t)ix->last_lane.load();
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
-    Lane& ln = ix->lanes[lane];
-    std::lock_guard<std::mutex> lk(ln.mu);
-    std::memset(out, 0, 8 * sizeof(uint32_t));
-    if (ln.last_nq != 0) std::memcpy(out, ln.last_kernel, sizeof(ln.last_kernel));
-    return IDB_OK;
+    return reinterpret_cast<Index*>(index)->last_search(lane, true, nullptr, out);
 }
 
 idb_status idb_last_search_counters(idb_index* index, uint64_t nq, uint64_t* out) {

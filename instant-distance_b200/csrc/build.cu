@@ -27,14 +27,14 @@ cudaError_t build_dispatch_ch6(const BuildArgs&, const BuildLaunch&, cudaStream_
 cudaError_t build_dispatch_ch8(const BuildArgs&, const BuildLaunch&, cudaStream_t);
 cudaError_t build_dispatch_long(const BuildArgs&, const BuildLaunch&, cudaStream_t);
 
-static cudaError_t build_dispatch_any(int ch, const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    switch (ch) {
+static cudaError_t build_dispatch_any(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
+    switch (kernel_ch(a.g.nchunks)) {
         case 1: return build_dispatch_ch1(a, l, st);
         case 2: return build_dispatch_ch2(a, l, st);
         case 3: return build_dispatch_ch3(a, l, st);
         case 4: return build_dispatch_ch4(a, l, st);
-        case 5: case 6: return build_dispatch_ch6(a, l, st);
-        case 7: case 8: return build_dispatch_ch8(a, l, st);
+        case 6: return build_dispatch_ch6(a, l, st);
+        case 8: return build_dispatch_ch8(a, l, st);
         default: return build_dispatch_long(a, l, st);
     }
 }
@@ -134,6 +134,13 @@ std::vector<std::pair<uint64_t, uint64_t>> layer_sizes(uint64_t n, uint32_t M, f
     return sizes;
 }
 
+// The build's control block, zeroed before every batch.
+struct BuildCtrl {
+    PassCtrl insert, retry;             // KA and its retry pass
+    unsigned long long relink_work;     // K2' work counter
+    uint32_t n_seg;                     // K2' work items: distinct target rows of the batch's link requests
+};
+
 struct BuildScratch {
     uint64_t* cand_keys = nullptr;
     uint32_t* cand_cnt = nullptr;
@@ -144,14 +151,12 @@ struct BuildScratch {
     uint32_t* fail_list = nullptr;
     void* cub_tmp = nullptr;
     size_t cub_bytes = 0;
-    // [0..8) KA work counter, [8..16) relink work counter, [16..20) n_seg, [20..24) KA fail count, [24..32) KA-retry work counter
-    // (all reset per batch); [32..36) inserts that failed even in the retry pass (never reset)
-    unsigned char* ctrl = nullptr;
-    uint32_t* h_fail = nullptr;     // pinned, 2 words: [0] failed even in the retry pass, [1] KA overflows of the last batch
+    BuildCtrl* ctrl = nullptr;
+    BuildCtrl* h_ctrl = nullptr;    // pinned: the last batch's control block
     ~BuildScratch() {
         cudaFree(cand_keys); cudaFree(cand_cnt); cudaFree(pairs); cudaFree(sorted); cudaFree(seg_start); cudaFree(status);
         cudaFree(fail_list); cudaFree(cub_tmp); cudaFree(ctrl);
-        if (h_fail) cudaFreeHost(h_fail);
+        if (h_ctrl) cudaFreeHost(h_ctrl);
     }
 };
 
@@ -239,13 +244,11 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     CUDA_TRY(cudaMalloc(&bs.seg_start, (size_t)max_batch * cap * 4));
     CUDA_TRY(cudaMalloc(&bs.status, (size_t)max_batch * 4));
     CUDA_TRY(cudaMalloc(&bs.fail_list, (size_t)max_batch * 4));
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&bs.h_fail), 8, cudaHostAllocDefault));
-    CUDA_TRY(cudaMalloc(&bs.ctrl, 64));
-    CUDA_TRY(cudaMemsetAsync(bs.ctrl, 0, 64, st));
+    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&bs.h_ctrl), sizeof(BuildCtrl), cudaHostAllocDefault));
+    CUDA_TRY(cudaMalloc(&bs.ctrl, sizeof(BuildCtrl)));
     CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, bs.cub_bytes, bs.pairs, bs.sorted, (int)(max_batch * cap), 0, 64, st));
     CUDA_TRY(cudaMalloc(&bs.cub_tmp, std::max<size_t>(bs.cub_bytes, 16)));
 
-    const int ch = (int)((ix->nchunks + 31) / 32);
     // Staging the kept rows in shared memory (72 KB per 2-warp CTA -> 6 warps per SM) trades 32 resident warps for 6 to save reads
     // that L1/L2 serve anyway, so it is off unless asked for.
     bool stage = false;
@@ -267,12 +270,12 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     a.cand_keys = bs.cand_keys;
     a.cand_cnt = bs.cand_cnt;
     a.pairs = bs.pairs;
-    a.status = bs.status;
-    a.fail_count = reinterpret_cast<uint32_t*>(bs.ctrl + 20);
-    a.fail_list = bs.fail_list;
+    a.work.status = bs.status;
+    a.work.fail_count = &bs.ctrl->insert.fail_count;
+    a.work.fail_list = bs.fail_list;
     a.sorted_pairs = bs.sorted;
     a.seg_start = bs.seg_start;
-    a.n_seg = reinterpret_cast<uint32_t*>(bs.ctrl + 16);
+    a.n_seg = &bs.ctrl->n_seg;
 
     for (uint32_t li = 0; li < num_layers; ++li) {  // lib.rs:304-329
         const uint32_t layer = num_layers - li - 1;
@@ -285,9 +288,10 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
             b = std::min<uint64_t>(b, end - g0);
             a.base = (uint32_t)g0;
             a.count = (uint32_t)b;
+            a.work.n_work = b;
             a.layer = layer;
             a.n_pairs_cap = (uint32_t)(b * cap);
-            CUDA_TRY(cudaMemsetAsync(bs.ctrl, 0, 32, st));
+            CUDA_TRY(cudaMemsetAsync(bs.ctrl, 0, sizeof(BuildCtrl), st));
             // KA: descent of every insert, then (device-side, normally a no-op) a retry pass with 2^18-slot hash sets and 64k-entry
             // tie lists for the inserts whose per-warp structures overflowed (e.g. inside a cluster of thousands of duplicate vectors)
             BuildLaunch l;
@@ -299,41 +303,22 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
             l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kSearchWarps - 1) / kSearchWarps, (uint64_t)ix->search_grid()));
             {
                 std::lock_guard<std::mutex> lk(ix->ctx->mu);  // the pool's tables must not be regrown under these launches
-                SearchArgs tier;
-                idb_status ts = ix->select_visited_tier(efc, tier, l.win);
+                idb_status ts = ix->select_visited_tier(efc, a.tier, l.win);
                 if (ts == IDB_OK) ts = ix->attach_window(ix->lanes[0], l.win);
                 if (ts != IDB_OK) return ts;
-                a.pool = tier.pool;
-                a.gslots = tier.gslots;
-                a.gshift = tier.gshift;
-                a.vis_mode = tier.vis_mode;
-                a.b16_cap_ids = tier.b16_cap_ids;
-                a.b16_nb = tier.b16_nb;
-                a.work_counter = reinterpret_cast<unsigned long long*>(bs.ctrl);
-                CUDA_TRY(build_dispatch_any(ch, a, l, st));
-                BuildArgs r = a;
+                a.work.work_counter = &bs.ctrl->insert.work_counter;
+                CUDA_TRY(build_dispatch_any(a, l, st));
                 BuildLaunch lr = l;
-                r.work_list = bs.fail_list;
-                r.n_work_dev = a.fail_count;
-                r.fail_list = nullptr;
-                r.fail_count = reinterpret_cast<uint32_t*>(bs.ctrl + 32);
-                r.work_counter = reinterpret_cast<unsigned long long*>(bs.ctrl + 24);
-                r.pool = ix->ctx->retry_pool();
-                r.gslots = kRetrySlots;
-                r.gshift = 32 - 18;
-                r.vis_mode = kVisHash;
                 lr.grid = kRetryCtas;
                 lr.win = LaunchWindow();
-                CUDA_TRY(build_dispatch_any(ch, r, lr, st));
+                CUDA_TRY(build_dispatch_any(retry_pass(a, *ix->ctx, &bs.ctrl->retry), lr, st));
             }
-            CUDA_TRY(cudaMemcpyAsync(bs.h_fail, bs.ctrl + 32, 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(bs.h_fail + 1, bs.ctrl + 20, 4, cudaMemcpyDeviceToHost, st));
-            const int ka_b16 = a.vis_mode == kVisB16 ? ix->b16_level : 0;
+            const int ka_b16 = a.tier.mode == kVisB16 ? ix->b16_level : 0;
             // K2: neighbour selection for the new nodes, own rows, link requests
             if (p.heuristic) {
                 l.op = kOpSelectNew;
                 l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
-                CUDA_TRY(build_dispatch_any(ch, a, l, st));
+                CUDA_TRY(build_dispatch_any(a, l, st));
             } else {
                 select_simple_kernel<<<(unsigned)std::min<uint64_t>(b, 1024), 64, 0, st>>>(a);
                 CUDA_TRY(cudaGetLastError());
@@ -342,19 +327,20 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
             size_t tmp = bs.cub_bytes;
             CUDA_TRY(cub::DeviceRadixSort::SortKeys(bs.cub_tmp, tmp, bs.pairs, bs.sorted, (int)(b * cap), 0, 64, st));
             segment_heads_kernel<<<(unsigned)((b * cap + 255) / 256), 256, 0, st>>>(bs.sorted, (uint32_t)(b * cap), bs.seg_start,
-                                                                                  reinterpret_cast<uint32_t*>(bs.ctrl + 16));
+                                                                                  &bs.ctrl->n_seg);
             CUDA_TRY(cudaGetLastError());
             // K2': re-prune every target row once
             l.op = p.heuristic ? kOpRelink : kOpRelinkSimple;
             l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b * cap + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
-            a.work_counter = reinterpret_cast<unsigned long long*>(bs.ctrl + 8);
-            CUDA_TRY(build_dispatch_any(ch, a, l, st));
+            a.work.work_counter = &bs.ctrl->relink_work;
+            CUDA_TRY(build_dispatch_any(a, l, st));
+            CUDA_TRY(cudaMemcpyAsync(bs.h_ctrl, bs.ctrl, sizeof(BuildCtrl), cudaMemcpyDeviceToHost, st));
             g0 += b;
             CUDA_TRY(cudaStreamSynchronize(st));  // fail fast: an insert that overflowed even the retry pass ends the build here
-            if (*bs.h_fail)
+            if (bs.h_ctrl->retry.fail_count)
                 return fail(IDB_ERR_CAPACITY, "%u inserts overflowed an internal per-insert structure (visited table / tie list) in the batch ending at %llu",
-                            *bs.h_fail, (unsigned long long)g0);
-            ix->note_overflows(efc, b, bs.h_fail[1], ka_b16);  // too many b16 overflows: later batches use a larger flavour
+                            bs.h_ctrl->retry.fail_count, (unsigned long long)g0);
+            ix->note_overflows(efc, b, bs.h_ctrl->insert.fail_count, ka_b16);  // too many b16 overflows: later batches use a larger flavour
             if (p.progress) p.progress(g0, n, p.progress_user);  // set_position (core:519-525)
         }
         if (layer != 0) {  // lib.rs:323-328

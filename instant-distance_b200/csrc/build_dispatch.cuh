@@ -15,15 +15,6 @@ struct BuildLaunch {
     LaunchWindow win;       // KA: persisting-L2 window on the b16 visited tables
 };
 
-template <int CH, int ROW_T, int EF_T, int B, class RT>
-cudaError_t launch_insert_search(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    const int smem = (WarpSmem<EF_T>::kBytes + (CH == 0 ? (int)long_q_bytes(a.g.nchunks) : 0)) * kSearchWarps;
-    auto kern = insert_search_kernel<CH, ROW_T, EF_T, B, RT>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    return launch_with_window(kern, l.grid, kSearchWarps * 32, smem, st, l.win, a);
-}
-
 template <int CH, int NB, bool kStage, class RT>
 cudaError_t launch_k2(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
     const int smem = (int)l.smem_per_warp * kBuildWarps;
@@ -45,15 +36,10 @@ template <int CH, int B, int NB, class RT>
 cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
     switch (l.op) {
         case kOpInsertSearch:
-            if (l.row_t <= 2) {
-                if (l.ef_t <= 4) return launch_insert_search<CH, 2, 4, B, RT>(a, l, st);
-                if (l.ef_t <= 8) return launch_insert_search<CH, 2, 8, B, RT>(a, l, st);
-                if (l.ef_t <= 16) return launch_insert_search<CH, 2, 16, B, RT>(a, l, st);
-                return launch_insert_search<CH, 2, 32, B, RT>(a, l, st);
-            }
-            if (l.ef_t <= 4) return launch_insert_search<CH, 4, 4, B, RT>(a, l, st);
-            if (l.ef_t <= 16) return launch_insert_search<CH, 4, 16, B, RT>(a, l, st);
-            return launch_insert_search<CH, 4, 32, B, RT>(a, l, st);
+            return with_tile(l.row_t, l.ef_t, [&](auto row, auto ef) {
+                constexpr int ROW_T = decltype(row)::value, EF_T = decltype(ef)::value;
+                return launch_traversal<CH, EF_T>(insert_search_kernel<CH, ROW_T, EF_T, B, RT>, a, 0, l.grid, st, l.win);
+            });
         case kOpSelectNew:
         case kOpRelink:
             if constexpr (CH > 0) {

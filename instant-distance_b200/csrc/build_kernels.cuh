@@ -33,17 +33,8 @@ struct BuildArgs {
     uint64_t* cand_keys;            // count x cand_cap : `nearest` of each insert, ascending
     uint32_t* cand_cnt;             // count
     uint64_t* pairs;                // count x 2M : (target << 32 | new), kKeyNone when unused
-    uint32_t* status;               // count
-    uint32_t* fail_count;
-    uint32_t* fail_list;            // KA: inserts whose visited table / tie list overflowed (null in the retry pass)
-    const uint32_t* work_list;      // retry pass: work item -> insert index of the batch
-    const uint32_t* n_work_dev;     // retry pass: number of work items, read on the device
-    unsigned long long* work_counter;
-    TablePool pool;                 // per-warp scratch tables, claimed per CTA (hnsw_device.cuh)
-    uint32_t gslots, gshift;
-    uint32_t vis_mode;
-    uint32_t b16_cap_ids;
-    uint32_t b16_nb;
+    TraversalWork work;             // KA: the batch's inserts (n_work = count); K2', simple relink: work_counter only
+    VisTier tier;                   // KA
     // relink
     const uint64_t* sorted_pairs;   // count*2M sorted ascending
     uint32_t n_pairs_cap;
@@ -177,44 +168,13 @@ struct SelectSmem {
 // ---------------------------------------------------------------------------------------------------------
 template <int CH, int ROW_T, int EF_T, int B, class RT>
 __global__ void __launch_bounds__(kSearchWarps * 32, kSearchCtasPerSm) insert_search_kernel(BuildArgs a) {  // same occupancy as K1
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    __shared__ uint32_t s_claim[2];
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const uint32_t n_work = a.n_work_dev ? *a.n_work_dev : a.count;
-    if (n_work == 0) return;  // the retry pass, normally
-
-    WarpState s;
-    WarpSmem<EF_T>::carve(s, smem_raw + (size_t)warp * WarpSmem<EF_T>::kBytes);
-    const uint32_t table0 = cta_tables_acquire(a.pool, s_claim, kSearchWarps);
-    bind_tables(s, a.pool, table0 + warp, a.gslots, a.gshift, a.vis_mode, a.b16_cap_ids, a.b16_nb);
-    vis_clear_small(s.vis, lane);
-
-    for (;;) {
-        unsigned long long wi = 0;
-        if (lane == 0) wi = atomicAdd(a.work_counter, 1ull);
-        wi = __shfl_sync(kFullMask, wi, 0);
-        if (wi >= n_work) break;
-        const uint32_t w = a.work_list ? a.work_list[wi] : (uint32_t)wi;
-        const uint32_t neu = a.base + w;
-        QVec<CH> q;
-        long_q_bind<EF_T>(q, smem_raw, a.g.nchunks, warp, kSearchWarps);
-        q_from_point<CH, RT>(q, a.g, neu, lane);
-        descend<CH, ROW_T, EF_T, B, false, RT>(a.g, s, q, a.layer, a.efc, lane, nullptr);
-        const uint64_t* near = s.near_base + s.cur * s.near_len;
-        const uint32_t len = s.status == kQueryOk ? s.cnt : 0u;
-        for (uint32_t j = lane; j < len; j += 32) a.cand_keys[(size_t)w * a.cand_cap + j] = near[j] & kKeyMask;
-        if (lane == 0) {
-            a.cand_cnt[w] = len;
-            a.status[w] = s.status;
-            if (s.status != kQueryOk) {
-                const uint32_t slot = atomicAdd(a.fail_count, 1u);
-                if (a.fail_list) a.fail_list[slot] = w;
-            }
-        }
-        finish_query(s, lane);
-    }
-    cta_tables_release(a.pool, s_claim);
+    traverse<CH, ROW_T, EF_T, B, RT, false, false, false, uint32_t>(
+        a.g, a.work, a.tier, a.layer, a.efc, nullptr,
+        [&](uint32_t w, QVec<CH>& q, int lane) { q_from_point<CH, RT>(q, a.g, a.base + w, lane); },
+        [&](uint32_t w, const uint64_t* near, uint32_t len, const WarpState&, int lane) {
+            for (uint32_t j = lane; j < len; j += 32) a.cand_keys[(size_t)w * a.cand_cap + j] = near[j] & kKeyMask;
+            if (lane == 0) a.cand_cnt[w] = len;
+        });
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -263,7 +223,7 @@ __global__ void __launch_bounds__(kBuildWarps * 32) relink_kernel(BuildArgs a, u
     const uint32_t n_seg = *a.n_seg;
     for (;;) {
         unsigned long long w = 0;
-        if (lane == 0) w = atomicAdd(a.work_counter, 1ull);
+        if (lane == 0) w = atomicAdd(a.work.work_counter, 1ull);
         w = __shfl_sync(kFullMask, w, 0);
         if (w >= n_seg) break;
         uint32_t pos = a.seg_start[w];
@@ -345,7 +305,7 @@ __global__ void __launch_bounds__(kBuildWarps * 32) relink_simple_kernel(BuildAr
     const uint32_t n_seg = *a.n_seg;
     for (;;) {
         unsigned long long w = 0;
-        if (lane == 0) w = atomicAdd(a.work_counter, 1ull);
+        if (lane == 0) w = atomicAdd(a.work.work_counter, 1ull);
         w = __shfl_sync(kFullMask, w, 0);
         if (w >= n_seg) break;
         uint32_t pos = a.seg_start[w];

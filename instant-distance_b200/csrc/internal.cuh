@@ -37,26 +37,54 @@ idb_status fail(idb_status st, const char* fmt, ...);
                                cudaGetErrorName(e__), __FILE__, __LINE__, cudaGetErrorString(e__));             \
     } while (0)
 
+// Float4 chunks per lane of the traversal instantiation that serves rows of `nchunks` chunks: 1, 2, 3, 4, 6 or 8, and 0 for rows of
+// more than 1024 elements (the long-row kernels, whose query lives in shared memory).
+constexpr int kernel_ch(uint32_t nchunks) {
+    const uint32_t c = (nchunks + 31) / 32;
+    return c <= 4 ? (int)c : c <= 6 ? 6 : c <= 8 ? 8 : 0;
+}
+
+// The big visited tier a traversal's warps bind (Index::select_visited_tier, DeviceCtx::retry_tier).
+struct VisTier {
+    TablePool pool;                    // per-warp scratch tables, claimed per CTA (hnsw_device.cuh)
+    uint32_t gslots, gshift;           // words in use per warp / hash flavour: 32 - log2(gslots)
+    uint32_t mode;                     // flavour (hnsw_device.cuh VisMode)
+    uint32_t b16_cap_ids;              // b16 flavour: ids per traversal before the retry pass takes over
+    uint32_t b16_nb;                   // b16 flavour: buckets in use over both segments
+};
+
+// The work items of one traversal pass (K1 or KA) and where it reports on them.
+struct TraversalWork {
+    unsigned long long n_work;         // number of work items ...
+    const uint32_t* n_work_dev;        // ... or, if non-null, read it from device memory (retry pass)
+    const uint32_t* work_list;         // optional indirection: work item -> query / insert index
+    unsigned long long* work_counter;
+    uint32_t* status;                  // per query / insert: QueryStatus
+    uint32_t* fail_count;
+    uint32_t* fail_list;               // items whose visited table / tie list overflowed; null in the retry pass
+};
+
+// Device-side counters of one traversal pass, zeroed before it.
+struct PassCtrl {
+    unsigned long long work_counter;
+    uint32_t fail_count;
+};
+// A search call's control block (Lane::ctrl).
+struct SearchCtrl {
+    PassCtrl main, retry;              // K1 and its retry pass
+    unsigned long long full_fetches;   // rows fetched in full (the rows the screen did not drop), by both passes
+};
+
 struct SearchArgs {
     GraphView g;
     const float4* queries;             // nq x nchunks float4 (zero padded rows)
-    unsigned long long n_work;         // number of work items ...
-    const uint32_t* n_work_dev;        // ... or, if non-null, read it from device memory (retry pass)
-    const uint32_t* work_list;         // optional indirection: work item -> query index
+    TraversalWork work;
     uint32_t ef, k;
     uint32_t* out_ids;
     float* out_dist;
     uint32_t* out_len;
     uint32_t* counters;                // nq x 4 u32 or null
-    uint32_t* status;                  // nq
-    unsigned long long* work_counter;
-    uint32_t* fail_count;
-    uint32_t* fail_list;               // may be null (retry pass)
-    TablePool pool;                    // per-warp scratch tables, claimed per CTA (hnsw_device.cuh)
-    uint32_t gslots, gshift;           // big visited tier: words in use per warp / hash flavour: 32 - log2(gslots)
-    uint32_t vis_mode;                 // flavour of the big visited tier (hnsw_device.cuh VisMode)
-    uint32_t b16_cap_ids;              // b16 flavour: ids per query before the retry pass takes over
-    uint32_t b16_nb;                   // b16 flavour: buckets in use over both segments
+    VisTier tier;
     uint64_t* out_keys;                // optional: nq x k packed (distance bits << 32 | id_map[pid]) for the sharded all-gather
     const uint32_t* id_map;            // optional: PointId -> caller's global row id
     int variant;                       // tuning variant of the kernel template (0 = default)
@@ -106,16 +134,32 @@ struct DeviceCtx {
     idb_status ensure_big(uint32_t stride_words);          // caller holds mu
     idb_status reserve_l2(size_t bytes);                    // caller holds mu
     TablePool main_pool(bool b16) const;
-    TablePool retry_pool() const;
+    VisTier retry_tier() const;                             // the retry pool's 2^18-slot hash sets
     ~DeviceCtx();
 };
+
+// The arguments of the retry pass behind a main traversal pass `a` (device-side, unconditional, normally a no-op): a few warps re-run
+// the items whose visited table or tie list overflowed, from a.work.fail_list, as many as the main pass counted on the device, with
+// the retry pool's tables.  Failures of the retry pass are only counted in ctrl->fail_count (and visible in status).
+template <class Args>
+Args retry_pass(const Args& a, const DeviceCtx& c, PassCtrl* ctrl) {
+    Args r = a;
+    r.work.n_work = 0;
+    r.work.n_work_dev = a.work.fail_count;
+    r.work.work_list = a.work.fail_list;
+    r.work.work_counter = &ctrl->work_counter;
+    r.work.fail_count = &ctrl->fail_count;
+    r.work.fail_list = nullptr;
+    r.tier = c.retry_tier();
+    return r;
+}
 
 // Per-call control state + host-API staging buffers; one per submission lane.  Calls on one lane are stream-ordered, so the
 // buffers are reused without waiting; calls on different lanes overlap on the device.
 struct Lane {
     std::mutex mu;
     cudaStream_t stream = nullptr;
-    unsigned char* ctrl = nullptr;   // [0..8) K1 work counter, [8..16) rows fetched in full, [16..20) K1 fail count, [32..40) retry work counter, [48..52) retry fail count
+    SearchCtrl* ctrl = nullptr;
     uint32_t* status = nullptr;   size_t status_cap = 0;
     uint32_t* fail_list = nullptr; size_t fail_cap = 0;
     uint32_t* counters = nullptr; size_t counters_cap = 0;
@@ -133,7 +177,7 @@ struct Lane {
     // host API: results land here first when the caller's output buffers are pageable (see HostOut in api.cu)
     unsigned char* h_out = nullptr; size_t h_out_cap = 0;   // pinned
     // asynchronous read-back of the control block of the lane's last call (how many queries overflowed the b16 tables)
-    uint32_t* h_ctrl = nullptr;      // pinned, 32 words: [0,16) the sampled overflow tally, [16,32) the host API's read-back
+    SearchCtrl* h_ctrl = nullptr;    // pinned, 2 blocks: [0] the sampled overflow tally, [1] the host API's read-back
     cudaEvent_t ev_ctrl = nullptr;
     bool ctrl_pending = false;
     int ctrl_b16 = 0;
@@ -218,9 +262,8 @@ struct Index {
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
     int search_grid() const;
-    // Fills the visited-tier fields of `a` (pool, gslots, ...) for a traversal with this ef and returns the launch window.
-    // Caller holds ctx->mu.
-    idb_status select_visited_tier(uint32_t ef, SearchArgs& a, LaunchWindow& win);
+    // The visited tier of a traversal with this ef, and its launch window.  Caller holds ctx->mu.
+    idb_status select_visited_tier(uint32_t ef, VisTier& tier, LaunchWindow& win);
     // The persisting-L2 window on the b16 tables rides on every launch as a launch attribute; it is ALSO kept as a stream attribute,
     // because profilers that replay a kernel (ncu) re-launch it without its launch attributes.
     idb_status attach_window(Lane& ln, const LaunchWindow& win);
@@ -230,6 +273,10 @@ struct Index {
     idb_status enqueue_search(Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
                               float* d_dist, uint32_t* d_len, uint64_t* out_keys);
     Lane& pick_lane();
+    // For the idb_last_search_* queries: under the lane's lock, what the lane's last search left behind — its control block (`ctrl`,
+    // once the lane's stream has drained) and its K1 instantiation (`kernel`, 8 words) — each optional, all zero when the lane has
+    // run none.  `latest`: lane 0xFFFFFFFF names the lane of the last call issued on this index.
+    idb_status last_search(uint32_t lane, bool latest, SearchCtrl* ctrl, uint32_t* kernel);
 };
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);

@@ -161,19 +161,10 @@ using namespace idb;
 
 extern "C" idb_status idb_last_search_full_fetches(idb_index* index, uint32_t lane, uint64_t* out_rows) {
     if (!index || !out_rows) return fail(IDB_ERR_INVALID_ARG, "null argument");
-    Index* ix = reinterpret_cast<Index*>(index);
-    if (lane == 0xFFFFFFFFu) lane = (uint32_t)ix->last_lane.load();
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
-    Lane& ln = ix->lanes[lane];
-    std::lock_guard<std::mutex> lk(ln.mu);
-    *out_rows = 0;
-    if (!ln.ctrl || ln.last_nq == 0) return IDB_OK;
-    CUDA_TRY(cudaSetDevice(ix->device));
-    uint64_t ctrl[8];
-    CUDA_TRY(cudaMemcpyAsync(ctrl, ln.ctrl, 64, cudaMemcpyDeviceToHost, ln.stream));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    *out_rows = ctrl[1];
-    return IDB_OK;
+    SearchCtrl c;
+    idb_status st = reinterpret_cast<Index*>(index)->last_search(lane, true, &c, nullptr);
+    if (st == IDB_OK) *out_rows = c.full_fetches;
+    return st;
 }
 
 extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* queries, uint64_t nq, const uint32_t* pairs, uint64_t npairs,
@@ -181,8 +172,8 @@ extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* quer
     if (!index || (npairs && (!queries || !pairs || !out_bound || !out_dist))) return fail(IDB_ERR_INVALID_ARG, "null argument");
     Index* ix = reinterpret_cast<Index*>(index);
     if (!ix->d_codes) return fail(IDB_ERR_UNSUPPORTED, "this index has no screening table (IDB_SCREEN=0, empty, or a non-finite value)");
-    const int ch = (int)((ix->nchunks + 31) / 32);
-    if (ch > 8) return fail(IDB_ERR_UNSUPPORTED, "dim %u: rows of more than 1024 elements are not screened", ix->dim);
+    const int ch = kernel_ch(ix->nchunks);
+    if (ch == 0) return fail(IDB_ERR_UNSUPPORTED, "dim %u: rows of more than 1024 elements are not screened", ix->dim);
     for (uint64_t i = 0; i < npairs; ++i)
         if (pairs[2 * i] >= nq || pairs[2 * i + 1] >= ix->n) return fail(IDB_ERR_INVALID_ARG, "pair %llu out of range", (unsigned long long)i);
     if (npairs == 0) return IDB_OK;
@@ -208,7 +199,7 @@ extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* quer
             case 2: e = launch_screen_bound<2>(g, q4, dp, npairs, dbound, ddist, st); break;
             case 3: e = launch_screen_bound<3>(g, q4, dp, npairs, dbound, ddist, st); break;
             case 4: e = launch_screen_bound<4>(g, q4, dp, npairs, dbound, ddist, st); break;
-            case 5: case 6: e = launch_screen_bound<6>(g, q4, dp, npairs, dbound, ddist, st); break;
+            case 6: e = launch_screen_bound<6>(g, q4, dp, npairs, dbound, ddist, st); break;
             default: e = launch_screen_bound<8>(g, q4, dp, npairs, dbound, ddist, st); break;
         }
     }

@@ -320,9 +320,9 @@ idb_status idb_sharded_search_batch_f32_multi(idb_index* const* shards, uint32_t
     uint32_t failed = 0;
     for (uint32_t i = 0; i < n_shards; ++i) {
         Lane& sl = reinterpret_cast<Index*>(shards[i])->lanes[0];
-        uint32_t ctrl[16] = {0};
-        if (sl.ctrl && sl.last_nq) CUDA_TRY(cudaMemcpy(ctrl, sl.ctrl, 64, cudaMemcpyDeviceToHost));
-        failed += ctrl[12];
+        SearchCtrl ctrl = {};
+        if (sl.ctrl && sl.last_nq) CUDA_TRY(cudaMemcpy(&ctrl, sl.ctrl, sizeof(ctrl), cudaMemcpyDeviceToHost));
+        failed += ctrl.retry.fail_count;
     }
     if (failed) return fail(IDB_ERR_CAPACITY, "%u queries overflowed an internal per-query structure on this rank's shards", failed);
     return IDB_OK;
