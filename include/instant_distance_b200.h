@@ -226,6 +226,13 @@ IDB_API idb_status idb_debug_gather_mix_bench(idb_index* index, uint32_t n_items
  * screening table (IDB_SCREEN=0, an empty index, a non-finite stored value, or rows of more than 1024 elements). */
 IDB_API idb_status idb_debug_screen_bound(idb_index* index, const float* queries, uint64_t nq, const uint32_t* pairs, uint64_t npairs,
                                           float* out_bound, float* out_dist);
+/* Test only: the sharded search's merge kernel, with the same launch, on keys (G x nq x k u64, host) the caller supplies: per query, the
+ * k smallest keys of its G lists (keys unique within a query; a slot of all ones is empty).  out_keys != NULL: the merged keys
+ * (nq x k, padded with all ones), as a rank's pre-merge writes them; otherwise out_ids / out_dist (nq x k, the low 32 bits of each key
+ * and its distance bits reported in the index's metric, padded with IDB_INVALID / +inf) and out_len (nq); out_dist / out_len may be
+ * NULL.  IDB_ERR_UNSUPPORTED when G x k keys do not fit the device's opt-in shared memory per block, like the sharded search. */
+IDB_API idb_status idb_debug_merge_topk(idb_index* index, const uint64_t* keys, uint32_t G, uint64_t nq, uint32_t k, uint32_t* out_ids,
+                                        float* out_dist, uint32_t* out_len, uint64_t* out_keys);
 
 IDB_API void* idb_index_stream(idb_index* index);      /* lane 0's cudaStream_t: builds, uploads and idb_search_batch_device run on it */
 IDB_API idb_status idb_index_sync(idb_index* index);   /* cudaStreamSynchronize on every lane of the index */

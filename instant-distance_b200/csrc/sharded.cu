@@ -178,6 +178,17 @@ namespace idb {
 idb_status search_device_keys(Index* ix, Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef_search, uint32_t k, uint32_t* d_ids,
                               uint64_t* d_keys);  // api.cu
 
+// The merge kernel holds one query's `lists` x k keys per warp in shared memory, so a merge of more than the device's opt-in shared
+// memory per block is refused.  *max_smem = that limit, for launch_merge.
+static idb_status merge_fits(const Index* ix, uint64_t lists, uint32_t k, int* max_smem) {
+    CUDA_TRY(cudaDeviceGetAttribute(max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ix->device));
+    if (lists * k * 8 > (uint64_t)*max_smem)
+        return fail(IDB_ERR_UNSUPPORTED, "%llu keys per query do not fit the merge kernel's shared memory (%d bytes)",
+                    (unsigned long long)(lists * k), *max_smem);
+    return IDB_OK;
+}
+
+// Warps per block: 4, halved while their keys do not fit max_smem; above 48 KB the kernel's dynamic shared-memory limit is raised.
 static idb_status launch_merge(Index* ix, cudaStream_t st, const uint64_t* keys, uint32_t G, uint64_t nq, uint32_t k, uint32_t* d_ids,
                                float* d_dist, uint32_t* d_len, uint64_t* d_keys, int max_smem) {
     const size_t per_warp = (size_t)G * k * 8;
@@ -202,11 +213,8 @@ static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, 
     CUDA_TRY(cudaSetDevice(ix->device));
     // merge kernels: world * k (and n_local * k) keys per query in shared memory; check the launches BEFORE anything is enqueued
     int max_smem = 0;
-    CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ix->device));
-    const uint64_t widest = std::max<uint64_t>((uint64_t)c->world, n_local) * k * 8;
-    if (widest > (uint64_t)max_smem)
-        return fail(IDB_ERR_UNSUPPORTED, "%llu keys per query do not fit the merge kernel's shared memory (%d bytes)",
-                    (unsigned long long)(widest / 8), max_smem);
+    idb_status st = merge_fits(ix, std::max<uint64_t>((uint64_t)c->world, n_local), k, &max_smem);
+    if (st != IDB_OK) return st;
     const size_t per = (size_t)nq * k;
     CUDA_TRY(ensure_u64(ln.keys_local, ln.keys_local_cap, per * (n_local > 1 ? n_local + 1 : 1)));
     CUDA_TRY(ensure_u64(ln.keys_all, ln.keys_all_cap, per * c->world));
@@ -216,7 +224,6 @@ static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, 
         CUDA_TRY(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
         CUDA_TRY(cudaEventRecord(fork, ln.stream));  // the queries (and anything else the caller enqueued) are ready
     }
-    idb_status st = IDB_OK;
     for (uint32_t i = 0; i < n_local && st == IDB_OK; ++i) {
         Index* sx = shards[i];
         Lane& sl = sx->lanes[0];
@@ -331,6 +338,43 @@ idb_status idb_sharded_search_batch_f32_multi(idb_index* const* shards, uint32_t
 idb_status idb_sharded_search_batch_f32(idb_index* index, idb_comm* comm, const float* queries, uint64_t nq, uint32_t ef_search, uint32_t k,
                                         uint32_t* out_ids, float* out_dist, uint32_t* out_len) {
     return idb_sharded_search_batch_f32_multi(&index, 1, comm, queries, nq, ef_search, k, out_ids, out_dist, out_len);
+}
+
+// The sharded search's merge (launch_merge: the same launch geometry and shared-memory limit) on keys the caller supplies.
+idb_status idb_debug_merge_topk(idb_index* index, const uint64_t* keys, uint32_t G, uint64_t nq, uint32_t k, uint32_t* out_ids,
+                                float* out_dist, uint32_t* out_len, uint64_t* out_keys) {
+    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    if (G == 0 || k == 0) return fail(IDB_ERR_INVALID_ARG, "G and k must be >= 1");
+    Index* ix = reinterpret_cast<Index*>(index);
+    std::lock_guard<std::mutex> lk(ix->lanes[0].mu);  // the merge runs on lane 0's stream
+    CUDA_TRY(cudaSetDevice(ix->device));
+    int max_smem = 0;
+    idb_status st = merge_fits(ix, G, k, &max_smem);
+    if (st != IDB_OK || nq == 0) return st;
+    if (!keys || (!out_keys && !out_ids)) return fail(IDB_ERR_INVALID_ARG, "null argument");
+    const size_t per = (size_t)nq * k, in_bytes = per * G * 8, out_bytes = out_keys ? per * 8 : per * 8 + nq * 4;
+    char* d = nullptr;
+    CUDA_TRY(cudaMalloc(&d, in_bytes + out_bytes));
+    uint64_t* d_in = reinterpret_cast<uint64_t*>(d);
+    uint64_t* d_keys = out_keys ? reinterpret_cast<uint64_t*>(d + in_bytes) : nullptr;
+    uint32_t* d_ids = out_keys ? nullptr : reinterpret_cast<uint32_t*>(d + in_bytes);
+    float* d_dist = out_keys || !out_dist ? nullptr : reinterpret_cast<float*>(d + in_bytes + per * 4);
+    uint32_t* d_len = out_keys || !out_len ? nullptr : reinterpret_cast<uint32_t*>(d + in_bytes + per * 8);
+    cudaStream_t s = ix->lanes[0].stream;
+    cudaError_t e = cudaMemcpyAsync(d_in, keys, in_bytes, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) st = launch_merge(ix, s, d_in, G, nq, k, d_ids, d_dist, d_len, d_keys, max_smem);
+    if (e == cudaSuccess && st == IDB_OK) {
+        if (out_keys) e = cudaMemcpyAsync(out_keys, d_keys, per * 8, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && d_ids) e = cudaMemcpyAsync(out_ids, d_ids, per * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && d_dist) e = cudaMemcpyAsync(out_dist, d_dist, per * 4, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && d_len) e = cudaMemcpyAsync(out_len, d_len, nq * 4, cudaMemcpyDeviceToHost, s);
+    }
+    const cudaError_t sync = cudaStreamSynchronize(s);  // before the buffer is freed, whatever happened above
+    cudaFree(d);
+    CUDA_TRY(e);
+    if (st != IDB_OK) return st;
+    CUDA_TRY(sync);
+    return IDB_OK;
 }
 
 }  // extern "C"

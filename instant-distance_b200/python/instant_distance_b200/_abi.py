@@ -24,7 +24,7 @@ SYMBOLS = [
     "idb_comm_unique_id", "idb_comm_create", "idb_comm_free", "idb_index_set_id_map", "idb_sharded_search_batch_f32",
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
-    "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel",
+    "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
 ]
 
 
@@ -83,6 +83,7 @@ def lib():
     L.idb_last_search_full_fetches.argtypes = [vp, C.c_uint32, u64p]
     L.idb_debug_screen_bound.argtypes = [vp, f32p, C.c_uint64, u32p, C.c_uint64, f32p, f32p]
     L.idb_last_search_kernel.argtypes = [vp, C.c_uint32, u32p]
+    L.idb_debug_merge_topk.argtypes = [vp, u64p, C.c_uint32, C.c_uint64, C.c_uint32, u32p, f32p, u32p, u64p]
     L.idb_index_num_lanes.restype = C.c_uint32
     L.idb_index_lane_stream.argtypes = [vp, C.c_uint32]
     L.idb_index_lane_stream.restype = vp
@@ -288,6 +289,24 @@ class Index:
         check(lib().idb_debug_screen_bound(self._h, ptr(q, C.c_float), q.shape[0], ptr(p, C.c_uint32), p.shape[0],
                                            ptr(bound, C.c_float), ptr(dist, C.c_float)))
         return bound, dist
+
+    def merge_topk(self, keys, k, premerge=False):
+        """The sharded search's merge kernel on keys (G x nq x k u64): the merged keys (nq x k) when `premerge`, else
+        (ids, dist, lens) with distances reported in this index's metric."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        G, nq, kk = keys.shape
+        if kk != k:
+            raise ValueError("keys must be G x nq x k")
+        if premerge:
+            out = np.empty((nq, k), dtype=np.uint64)
+            check(lib().idb_debug_merge_topk(self._h, ptr(keys, C.c_uint64), G, nq, k, None, None, None, ptr(out, C.c_uint64)))
+            return out
+        ids = np.empty((nq, k), dtype=np.uint32)
+        dist = np.empty((nq, k), dtype=np.float32)
+        lens = np.empty(nq, dtype=np.uint32)
+        check(lib().idb_debug_merge_topk(self._h, ptr(keys, C.c_uint64), G, nq, k, ptr(ids, C.c_uint32), ptr(dist, C.c_float),
+                                         ptr(lens, C.c_uint32), None))
+        return ids, dist, lens
 
     def last_failures(self, lane=0):
         out = C.c_uint32()

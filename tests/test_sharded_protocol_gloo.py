@@ -11,7 +11,7 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from tests import datagen
+from tests import datagen, merge_statement
 
 
 def _free_port():
@@ -98,6 +98,46 @@ def test_merge_keys_pads_and_orders():
     assert ids.tolist() == [[3, 7, 2, 9]] and dist.tolist() == [[0.25, 0.5, 1.0, 1.0]] and lens.tolist() == [4]
     ids, dist, lens = sharded.merge_keys(keys, 6)
     assert ids[0].tolist() == [3, 7, 2, 9, 5, 0xFFFFFFFF] and lens.tolist() == [5] and np.isinf(dist[0][5])
+
+
+@pytest.mark.parametrize("kind", merge_statement.KINDS + ("mixed",))
+@pytest.mark.parametrize("G,nq,k", [(1, 5, 1), (2, 7, 2), (3, 9, 31), (7, 5, 33), (8, 4, 100), (64, 3, 32)])
+def test_merge_keys_equals_the_plain_statement(kind, G, nq, k):
+    """The host statement of the merge (sharded.merge_keys, used by the GPU tests and bench.py) against the plain one, on the
+    adversarial key sets the merge kernel is checked on: ties across lists at the k boundary, empty and partial lists, unordered
+    lists, distance bits 0 / subnormal / +inf / NaN and global ids 0 and 0xFFFFFFFE."""
+    from instant_distance_b200 import sharded
+
+    keys = merge_statement.mixed(G, nq, k, 7) if kind == "mixed" else merge_statement.keyset(kind, G, nq, k, 7)
+    ids, dist, lens = sharded.merge_keys(keys, k)
+    w_ids, w_dist, w_lens = merge_statement.merge(keys, k)
+    assert (ids == w_ids).all() and dist.tobytes() == w_dist.tobytes() and (lens == w_lens).all()
+
+
+def test_merge_key_sets_are_what_they_claim():
+    """Keys are unique within a query, and each kind holds the cases it is there for."""
+    ms = merge_statement
+    for kind in ms.KINDS:
+        keys = ms.keyset(kind, 3, 9, 5, 1)
+        for q in range(9):
+            real = [int(x) for x in keys[:, q, :].ravel() if int(x) != ms.KEY_NONE]
+            assert len(set(real)) == len(real)
+    prefix = ms.keyset("prefix", 3, 9, 5, 1)
+    assert (prefix[:, 0, :] == np.uint64(ms.KEY_NONE)).all() and (prefix[:, 1, :] != np.uint64(ms.KEY_NONE)).all()
+    ties = ms.keyset("ties", 3, 2, 5, 1)
+    d, g = ties >> np.uint64(32), ties & np.uint64(0xFFFFFFFF)
+    assert (d == d[:1, :, :1]).all() and (g[0].min(axis=1) > g[1].max(axis=1)).all()  # list 0 holds the highest ids
+    special = ms.keyset("special", 2, 50, 8, 1)
+    dbits = set((special >> np.uint64(32)).ravel().tolist())
+    assert {0, ms.SUBNORMAL, ms.INF, ms.QNAN} <= dbits
+    gids = special & np.uint64(0xFFFFFFFF)
+    assert ((gids == 0).any(axis=(0, 2)) & (gids == 0xFFFFFFFE).any(axis=(0, 2))).all()
+    # the cosine report halves the distance and keeps NaN and +inf
+    keys = np.array([[(0x40000000 << 32) | 5, (ms.QNAN << 32) | 6, ms.KEY_NONE]], dtype=np.uint64)
+    _, dist, lens = ms.report(keys, "cosine")
+    assert dist.view(np.uint32).tolist() == [[0x3F800000, ms.QNAN, ms.INF]] and lens.tolist() == [2]
+    _, dist, _ = ms.report(np.array([[(ms.SUBNORMAL << 32) | 1]], dtype=np.uint64), "cosine")
+    assert dist.view(np.uint32).tolist() == [[0]]  # half the smallest subnormal rounds to even: 0
 
 
 def test_merge_orders_exact_ties_by_global_id():
