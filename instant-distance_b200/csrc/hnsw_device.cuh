@@ -564,9 +564,34 @@ __device__ __forceinline__ bool vis_reserve(VisitedSet& v, uint32_t incoming, in
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// K1 phase clock (compile-time switch IDB_K1_PHASES, off in the product build; scripts/k1_phases.py builds a copy with it on).
+// search_layer adds clock64() deltas per warp to one tally per phase of an expansion; a phase ends where its loads have been
+// consumed, so a tally holds the phase's issue AND the wait for its own loads.  Each search_layer call of K1 adds its tallies to
+// g_k1_phases (one copy per translation unit: search_ch1.cu's is read by idb_debug_k1_phases).
+// ---------------------------------------------------------------------------------------------------------
+#ifdef IDB_K1_PHASES
+enum K1Phase : int {
+    kPhPop, kPhAdj, kPhVisit, kPhScreenLoad, kPhScreenMath, kPhGather, kPhMerge, kPhTies, kPhCount,
+    // event counts behind the cycle tallies
+    kPhExpansions = kPhCount, kPhScreenBatches, kPhSlots
+};
+static __device__ unsigned long long g_k1_phases[kPhSlots];
+#define IDB_PHASE(s, k) k1_phase_mark(s, k)
+#define IDB_PHASE_COUNT(s, k, n) ((s).ph[k] += (n))
+#else
+#define IDB_PHASE(s, k) ((void)0)
+#define IDB_PHASE_COUNT(s, k, n) ((void)0)
+#endif
+
+// ---------------------------------------------------------------------------------------------------------
 // Per-warp traversal state.
 // ---------------------------------------------------------------------------------------------------------
 struct WarpState {
+#ifdef IDB_K1_PHASES
+    uint32_t ph[kPhSlots];       // this search_layer call's tallies (warp-uniform)
+    long long ph_t;              // clock64() at the end of the last phase
+    uint32_t ph_sink;            // keeps the loads a phase waits for from being optimised away
+#endif
     uint64_t* near_base;     // shared: two buffers of near_len keys each (ping-pong for the merge)
     uint32_t near_len;       // 32*EF_T
     uint32_t* cpid;          // shared: 128 compacted new ids of the current row
@@ -585,6 +610,29 @@ struct WarpState {
     uint32_t n_full;             // rows fetched in full over the whole descent (n_dist minus what the screen dropped)
     VisitedSet vis;
 };
+
+#ifdef IDB_K1_PHASES
+__device__ __forceinline__ void k1_phase_mark(WarpState& s, int k) {
+    const long long t = clock64();
+    s.ph[k] += (uint32_t)(t - s.ph_t);
+    s.ph_t = t;
+}
+// Wait for x (a value a phase loaded) before the phase is closed: a vote consumes it.
+__device__ __forceinline__ void k1_phase_wait(WarpState& s, uint32_t x) { s.ph_sink ^= __ballot_sync(kFullMask, x == 0x9E3779B9u); }
+__device__ __forceinline__ void k1_phase_begin(WarpState& s) {
+#pragma unroll
+    for (int k = 0; k < kPhSlots; ++k) s.ph[k] = 0;
+    s.ph_sink = 0;
+    s.ph_t = clock64();
+}
+__device__ __forceinline__ void k1_phase_flush(WarpState& s, int lane) {
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < kPhSlots; ++k) atomicAdd(&g_k1_phases[k], (unsigned long long)s.ph[k]);
+        if (s.ph_sink == 0xFFFFFFFFu) atomicAdd(&g_k1_phases[kPhTies], 0ull);  // (never: a use of the sink)
+    }
+}
+#endif
 
 __device__ __forceinline__ uint32_t lower_bound_keys(const uint64_t* a, uint32_t n, uint64_t key) {
     uint32_t lo = 0, hi = n;
@@ -734,25 +782,43 @@ __device__ __forceinline__ constexpr int screen_rows() { return CH == 1 ? 32 : C
 // Drops the candidates in cpid[0, n_new) whose bound exceeds fdist (the distance of the ef-th key of nearest) and compacts the rest,
 // in row order, to the front of cpid.  Returns how many are left.  Warp-uniform call.
 template <int CH, bool kFull>
-__device__ __forceinline__ uint32_t screen_candidates(const GraphView& g, const float4 (&q)[CH], uint32_t* cpid, uint32_t n_new, float fdist,
+__device__ __forceinline__ uint32_t screen_candidates(WarpState& s, const GraphView& g, const float4 (&q)[CH], uint32_t n_new, float fdist,
                                                       int lane) {
+    uint32_t* cpid = s.cpid;
     constexpr int NS = screen_rows<CH>();
     bool cok[CH];
 #pragma unroll
     for (int j = 0; j < CH; ++j) cok[j] = kFull || (uint32_t)(lane + 32 * j) < g.nchunks;
-    const uint32_t* lane_codes = g.codes + lane;
+    // The lane's base address and the row stride stay in registers (as in batch_distances_impl): each row address is then ONE
+    // IMAD.WIDE, where re-reading g.codes / g.nchunks for every predicated row cost about a dozen instructions per row.
+    const char* lane_codes = reinterpret_cast<const char*>(g.codes + lane);
+    asm volatile("" : "+l"(lane_codes));
+    uint32_t row_bytes = kFull ? 32u * CH * 4u : g.nchunks * 4u;
+    if (!kFull) asm volatile("" : "+r"(row_bytes));
     uint32_t kept = 0;
 #pragma unroll 1
     for (uint32_t b0 = 0; b0 < n_new; b0 += NS) {
         const uint32_t nb = n_new - b0;
+        IDB_PHASE_COUNT(s, kPhScreenBatches, 1u);
         uint32_t w[NS][CH];
 #pragma unroll
         for (int i = 0; i < NS; ++i) {
             const bool ok = (uint32_t)i < nb;
-            const uint32_t* row = lane_codes + (size_t)cpid[b0 + i] * g.nchunks;  // (entries past n_new are stale ids: never loaded)
+            const char* row = lane_codes + (size_t)cpid[b0 + i] * row_bytes;  // (entries past n_new are stale ids: never loaded)
 #pragma unroll
-            for (int j = 0; j < CH; ++j) w[i][j] = (ok && cok[j]) ? __ldg(row + 32 * j) : 0u;
+            for (int j = 0; j < CH; ++j) w[i][j] = (ok && cok[j]) ? __ldg(reinterpret_cast<const uint32_t*>(row + 128 * j)) : 0u;
         }
+#ifdef IDB_K1_PHASES
+        {
+            uint32_t x = 0;
+#pragma unroll
+            for (int i = 0; i < NS; ++i)
+#pragma unroll
+                for (int j = 0; j < CH; ++j) x ^= w[i][j];
+            k1_phase_wait(s, x);
+            IDB_PHASE(s, kPhScreenLoad);
+        }
+#endif
         const uint32_t mine = (uint32_t)lane < (uint32_t)NS && (uint32_t)lane < nb ? cpid[b0 + lane] : kInvalid;
         float p[NS];
 #pragma unroll
@@ -769,6 +835,7 @@ __device__ __forceinline__ uint32_t screen_candidates(const GraphView& g, const 
         __syncwarp();  // every lane has read this batch's ids before any is overwritten (writes go to [kept, b0 + NS))
         if (keep) cpid[kept + __popc(m & ((1u << lane) - 1u))] = mine;
         kept += __popc(m);
+        IDB_PHASE(s, kPhScreenMath);
     }
     __syncwarp();
     return kept;
@@ -913,6 +980,9 @@ template <int CH, int ROW_T, int EF_T, int B, bool kLive, class RT, bool FULL, b
 __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, const QVec<CH>& q, const uint32_t* rows,
                                              uint32_t width, uint32_t links, uint32_t ef_cur, bool seed_entry, int lane) {
     const uint32_t lt_mask = (1u << lane) - 1;
+#ifdef IDB_K1_PHASES
+    k1_phase_begin(s);
+#endif
     for (;;) {
         uint64_t* near = (s.near_base + s.cur * s.near_len);
         uint32_t n_new = 0;
@@ -958,6 +1028,8 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
                 break;  // heap empty, or its min is strictly beyond the furthest result (lib.rs:601-603)
             }
             s.n_expand++;
+            IDB_PHASE(s, kPhPop);
+            IDB_PHASE_COUNT(s, kPhExpansions, 1u);
 
             // ---- row of the candidate: NearestIter stops at the first INVALID (types.rs:178-191) ----------
             uint32_t ent[ROW_T];
@@ -974,6 +1046,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
                 uint32_t m = __ballot_sync(kFullMask, ent[t] == kInvalid);
                 if (m) count = 32 * t + __ffs(m) - 1;
             }
+            IDB_PHASE(s, kPhAdj);
             if (count == 0) continue;
 
             // ---- visited.insert for every row entry (lib.rs:705), compacted in row order ------------------
@@ -1013,13 +1086,14 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
             }
             s.vis.count += n_new;
             s.n_dist += n_new;
+            IDB_PHASE(s, kPhVisit);
             if (n_new == 0) continue;
             __syncwarp();
             // ---- screen (DESIGN §4): with nearest full, a candidate whose code bound exceeds the furthest distance has a key
             // above the furthest key, so it would not be admitted; only the others are fetched in full, still in row order --------
             if constexpr (SCREEN && CH > 0 && !kLive && !TMA) {
                 if (g.codes && s.cnt >= ef_cur) {
-                    n_new = screen_candidates<CH, FULL>(g, q.r, s.cpid, n_new, __uint_as_float(key_dbits(near[s.cnt - 1])), lane);
+                    n_new = screen_candidates<CH, FULL>(s, g, q.r, n_new, __uint_as_float(key_dbits(near[s.cnt - 1])), lane);
                     if (n_new == 0) continue;
                 }
             }
@@ -1035,6 +1109,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
             const uint32_t c = 32 * gi + lane;
             keyg[gi] = c < n_new ? s.ckey[c] : kKeyNone;
         }
+        IDB_PHASE(s, kPhGather);
 
         // ---- admission (lib.rs:712-719): A = entries with rank_S < ef ----------------------------------
         const bool full = s.cnt >= ef_cur;
@@ -1052,6 +1127,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
             }
             nA += __popc(__ballot_sync(kFullMask, inA[gi]));
         }
+        IDB_PHASE(s, kPhMerge);
         if (nA == 0) continue;
 
         // ---- merge S and A into the other buffer: pos = rank among the union ---------------------------
@@ -1103,6 +1179,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
         const uint32_t total = old_cnt + nA;
         s.cnt = min(total, ef_cur);
         s.cur ^= 1;
+        IDB_PHASE(s, kPhMerge);
 
         // ---- candidates that fell off the end (lib.rs:612 truncate) -------------------------------------
         if (total > ef_cur) {
@@ -1122,9 +1199,13 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
                 maybe |= inA[gi] && (rank[gi] + less[gi] >= ef_cur) && key_dbits(keyg[gi]) == fbits;
             if (__any_sync(kFullMask, maybe))
                 collect_ties<ROW_T, EF_T>(s, near, old_cnt, shift, keyg, rank, inA, less, ef_cur, fbits, lane);
+            IDB_PHASE(s, kPhTies);
             if (s.status != kQueryOk) break;
         }
     }
+#ifdef IDB_K1_PHASES
+    k1_phase_flush(s, lane);
+#endif
 }
 
 // Search::cull (lib.rs:729-737): candidates := nearest; visited := {pids of nearest}.

@@ -21,3 +21,17 @@ cudaError_t dispatch_search_ch1(const SearchArgs& a, int row_t, int ef_t, int gr
     return dispatch_row_ef<1, 16>(a, row_t, ef_t, grid, st, win);
 }
 }  // namespace idb
+
+#ifdef IDB_K1_PHASES
+// The phase tallies of this translation unit's K1 kernels (hnsw_device.cuh, "K1 phase clock"): copies kPhSlots u64 to out, then zeroes
+// them when reset != 0.  Only in a library built with -DIDB_K1_PHASES (scripts/k1_phases.py).
+extern "C" __attribute__((visibility("default"))) int idb_debug_k1_phases(unsigned long long* out, int reset) {
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (cudaMemcpyFromSymbol(out, idb::g_k1_phases, sizeof(idb::g_k1_phases)) != cudaSuccess) return -1;
+    if (reset) {
+        static const unsigned long long zero[idb::kPhSlots] = {};
+        if (cudaMemcpyToSymbol(idb::g_k1_phases, zero, sizeof(zero)) != cudaSuccess) return -1;
+    }
+    return idb::kPhSlots;
+}
+#endif
