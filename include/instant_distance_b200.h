@@ -150,6 +150,22 @@ IDB_API idb_status idb_search_batch_device(idb_index* index, const float* d_quer
  * issued alternately on two lanes keep the GPU full across batch boundaries. */
 IDB_API idb_status idb_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq, uint32_t ef_search,
                                         uint32_t k, uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len);
+
+/* Exact k-NN: for each query, the min(k, n) smallest (canonical distance, PointId) over ALL stored rows, in the index's metric and
+ * row type; same output layout, padding, id map and distance reporting as idb_search_batch_f32.  1 <= k <= 1024.
+ * Takes an idle submission lane, like idb_search_batch_f32 (any number of host threads, alongside approximate searches).
+ * Ties are broken by the lower PointId and NaN distances order last, so the answer is unique and bit-reproducible: the ground truth
+ * to measure an approximate search's recall against (DESIGN.md §9a).  Exact calls leave the approximate-search diagnostics
+ * (idb_last_search_counters / _failures / _retried / _full_fetches / _kernel, idb_index_last_kernel_ms) describing the last
+ * approximate search.  Null index / queries (nq > 0) / out_ids or k == 0: IDB_ERR_INVALID_ARG; k > 1024: IDB_ERR_UNSUPPORTED;
+ * nq == 0: IDB_OK, nothing written. */
+IDB_API idb_status idb_exact_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, uint32_t k,
+                                              uint32_t* out_ids, float* out_dist, uint32_t* out_len);
+/* Same, device pointers on the index's device (d_queries: nq x dim at any alignment), enqueued on submission lane `lane` without
+ * syncing (lane >= idb_index_num_lanes(): IDB_ERR_INVALID_ARG). */
+IDB_API idb_status idb_exact_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq,
+                                                      uint32_t k, uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len);
+
 IDB_API uint32_t idb_index_num_lanes(void);
 IDB_API void* idb_index_lane_stream(idb_index* index, uint32_t lane);  /* cudaStream_t of that lane */
 /* Waits for the last call on `lane` and reports how many of its queries failed even in the retry pass (0 = all results valid). */

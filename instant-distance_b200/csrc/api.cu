@@ -364,7 +364,7 @@ void HostOut::finish() const {
 void Lane::free_all() {
     cudaFree(ctrl); cudaFree(status); cudaFree(fail_list); cudaFree(counters);
     cudaFree(q); cudaFree(qn); cudaFree(ids); cudaFree(dist); cudaFree(len);
-    cudaFree(keys_local); cudaFree(keys_all); cudaFree(q2); cudaFree(ids2);
+    cudaFree(keys_local); cudaFree(keys_all); cudaFree(q2); cudaFree(ids2); cudaFree(exact_keys);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (ev_ctrl) cudaEventDestroy(ev_ctrl);
@@ -676,6 +676,7 @@ idb_status Index::init_device(int dev) {
     if (const char* e = std::getenv("IDB_B16_BYTES")) b16_bytes_override = (uint32_t)std::max(64, std::atoi(e));
     if (const char* e = std::getenv("IDB_VIS_SLOTS")) vis_slots_override = next_pow2((uint64_t)std::max(64, std::atoi(e)));
     if (const char* e = std::getenv("IDB_SCREEN")) screen = std::atoi(e) != 0;
+    if (const char* e = std::getenv("IDB_EXACT_SCRATCH_KEYS")) exact_scratch_keys = (uint64_t)std::max(1LL, std::atoll(e));
     return IDB_OK;
 }
 

@@ -1,0 +1,368 @@
+// exact.cu — exact k-nearest-neighbour search: for every query, the k smallest keys (canonical distance bits << 32 | PointId) over ALL
+// stored rows (DESIGN.md §9a).
+//
+// A warp holds QW queries in registers (lane l owns chunks l, l+32, ... of each, as in K1) and streams the rows of one slice of the
+// index NB at a time; every distance comes from lane_partial + batch_butterfly, the helpers K1 computes its distances with, so the
+// two agree bit for bit.  Each (query, slice) keeps a sorted list of its k smallest keys in global scratch; a new key is compared with
+// the list's k-th key and almost always rejected there.  Slices split the rows when the queries alone do not fill the device; their
+// lists are merged by K4 (merge.cu).
+#include <algorithm>
+#include <cstring>
+
+#include "internal.cuh"
+
+namespace idb {
+
+namespace {
+
+constexpr uint32_t kExactMaxK = 1024;
+constexpr int kExactWarps = 8;                 // warps per CTA: they walk the same rows in the same order (L1 serves the others)
+constexpr uint64_t kExactScratchKeys = 1ull << 25;  // keys of per-call list scratch (256 MB): larger batches run in query chunks
+constexpr uint32_t kExactMaxSliceKeys = 2048;  // slices x k: K4's cost grows with its square
+constexpr uint64_t kExactMinSliceRows = 1024;
+
+// Queries per warp (QW) and rows per step (NB) of each CH: about 32 registers of query and 32-64 of rows per lane.
+template <int CH>
+struct ExactShape {
+    static constexpr int QW = CH == 1 ? 8 : CH == 2 ? 4 : (CH == 3 || CH == 4 || CH == 6) ? 2 : 1;
+    static constexpr int NB = CH == 0 ? kLongRowsInFlight : CH == 1 ? 8 : CH <= 3 ? 4 : 2;
+};
+
+struct ExactArgs {
+    GraphView g;
+    const float4* queries;      // nq x nchunks (zero padded, 16-byte aligned)
+    uint64_t nq;                // queries of this chunk
+    uint32_t k;
+    uint32_t S;                 // slices
+    uint64_t slice_rows;        // rows per slice (the last one may be shorter or empty)
+    uint64_t* lists;            // S x nq x k keys
+    // S == 1: the scan kernel writes the results itself
+    uint32_t* out_ids;
+    float* out_dist;
+    uint32_t* out_len;
+    const uint32_t* id_map;
+    uint32_t metric;
+};
+
+// Adds the keys of the lanes in m (distinct, each below the list's k-th key) to the sorted list L of cnt <= k keys.  New position of
+// an old entry: its index + #{new keys below it}; of a new key: lower_bound in L + #{new keys below it} (K1's rank rule).  Entries
+// only move up, so the old ones are moved top down, 32 at a time, each chunk read before it is written.  Returns the new k-th key
+// (kKeyNone while the list holds fewer than k).  Warp-uniform call.
+__device__ __forceinline__ uint64_t list_insert(uint64_t* L, uint32_t& cnt, uint32_t k, uint64_t key, uint32_t m, int lane) {
+    const bool in = (m >> lane) & 1u;
+    uint32_t r = 0;
+    uint64_t kmin = kKeyNone;
+    for (uint32_t mm = m; mm; mm &= mm - 1) {
+        const uint64_t o = shfl64(key, __ffs(mm) - 1);
+        r += o < key ? 1u : 0u;
+        kmin = o < kmin ? o : kmin;
+    }
+    const uint32_t lo = lower_bound_keys(L, cnt, kmin);
+    const uint32_t pos = in ? lower_bound_keys(L, cnt, key) + r : k;
+    if (cnt > lo) {
+        for (int32_t base = (int32_t)((cnt - 1) & ~31u); base >= (int32_t)(lo & ~31u); base -= 32) {
+            const uint32_t idx = (uint32_t)base + lane;
+            const bool have = idx >= lo && idx < cnt;
+            const uint64_t x = have ? L[idx] : kKeyNone;
+            uint32_t s = 0;
+            for (uint32_t mm = m; mm; mm &= mm - 1) s += shfl64(key, __ffs(mm) - 1) < x ? 1u : 0u;
+            __syncwarp();
+            if (have && idx + s < k) L[idx + s] = x;
+            __syncwarp();
+        }
+    }
+    if (in && pos < k) L[pos] = key;
+    __syncwarp();
+    cnt = min(k, cnt + (uint32_t)__popc(m));
+    return cnt == k ? L[k - 1] : kKeyNone;
+}
+
+template <int CH, class RT>
+__global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs a) {
+    constexpr int QW = ExactShape<CH>::QW, NB = ExactShape<CH>::NB;
+    static_assert(CH > 0 || QW == 1, "long rows: one query per warp (it lives in shared memory)");
+    extern __shared__ float4 sm_exact_q[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpc = blockDim.x >> 5;
+    const uint64_t q0 = ((uint64_t)blockIdx.x * wpc + warp) * QW;
+    if (q0 >= a.nq) return;
+    const uint32_t nchunks = a.g.nchunks;
+    const uint64_t r0 = min(a.g.n, (uint64_t)blockIdx.y * a.slice_rows), r1 = min(a.g.n, r0 + a.slice_rows);
+
+    QVec<CH> q[QW];
+    uint64_t* L[QW];
+    uint32_t cnt[QW];
+    uint64_t thr[QW];  // the list's k-th key; 0 for a slot past the batch (no key is below it)
+#pragma unroll
+    for (int j = 0; j < QW; ++j) {
+        const uint64_t qi = q0 + j < a.nq ? q0 + j : q0;
+        L[j] = a.lists + ((size_t)blockIdx.y * a.nq + qi) * a.k;
+        cnt[j] = 0;
+        thr[j] = q0 + j < a.nq ? kKeyNone : 0ull;
+        if constexpr (CH == 0) {
+            q[j].ngroups = (nchunks + 31) / 32;
+            q[j].s = sm_exact_q + (size_t)warp * q[j].ngroups * 32;
+        }
+        q_from_f32<CH>(q[j], a.queries + qi * nchunks, nchunks, lane);
+    }
+
+    const uint32_t row_bytes = nchunks * RT::kChunkBytes;
+    const char* lane_base = a.g.points + lane * RT::kChunkBytes;
+    const bool mine_lane = lane < NB;
+#pragma unroll 1
+    for (uint64_t b0 = r0; b0 < r1; b0 += NB) {
+        const uint32_t nb = r1 - b0 < (uint64_t)NB ? (uint32_t)(r1 - b0) : (uint32_t)NB;
+        float d[QW];
+        if constexpr (CH == 0) {  // batch_distances_long's order: four chains per row carried across groups of 32 chunks
+            const char* row[NB];
+            float4 acc[NB];
+#pragma unroll
+            for (int i = 0; i < NB; ++i) {
+                row[i] = lane_base + (size_t)(b0 + ((uint32_t)i < nb ? i : 0)) * row_bytes;
+                acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll 1
+            for (uint32_t j = 0; j < q[0].ngroups; ++j) {
+                const bool ok = lane + 32u * j < nchunks;
+                const float4 qq = q[0].s[lane + 32u * j];
+                typename RT::Raw v[NB];
+#pragma unroll
+                for (int i = 0; i < NB; ++i) v[i] = (ok && (uint32_t)i < nb) ? RT::ld_raw(row[i] + (size_t)j * 32 * RT::kChunkBytes) : RT::zero();
+#pragma unroll
+                for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, RT::widen(v[i]));
+            }
+            float p[NB];
+#pragma unroll
+            for (int i = 0; i < NB; ++i) p[i] = lane_sum(acc[i]);
+            d[0] = batch_butterfly<NB>(p, lane);
+        } else {  // batch_distances_impl's order, the rows shared by the warp's QW queries
+            typename RT::Raw v[NB][CH];
+#pragma unroll
+            for (int i = 0; i < NB; ++i) {
+                const bool ok = (uint32_t)i < nb;
+                const char* row = lane_base + (size_t)(b0 + (ok ? i : 0)) * row_bytes;
+#pragma unroll
+                for (int j = 0; j < CH; ++j)
+                    v[i][j] = (ok && (uint32_t)(lane + 32 * j) < nchunks) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
+            }
+#pragma unroll
+            for (int qj = 0; qj < QW; ++qj) {
+                float p[NB];
+#pragma unroll
+                for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(q[qj].r, v[i]);
+                d[qj] = batch_butterfly<NB>(p, lane);  // lane l: row b0 + (l & (NB - 1))
+            }
+        }
+        const uint32_t pid = (uint32_t)(b0 + (lane & (NB - 1)));
+        const bool mine = mine_lane && (uint32_t)lane < nb;
+#pragma unroll
+        for (int qj = 0; qj < QW; ++qj) {
+            const uint64_t key = mk_key(d[qj], pid);
+            const uint32_t m = __ballot_sync(kFullMask, mine && key < thr[qj]);
+            if (m) thr[qj] = list_insert(L[qj], cnt[qj], a.k, key, m, lane);
+        }
+    }
+
+#pragma unroll
+    for (int j = 0; j < QW; ++j) {
+        const uint64_t qi = q0 + j;
+        if (qi >= a.nq) break;
+        if (a.S == 1) {  // K1's epilogue: ids through the id map, distances as the metric reports them, padding
+            for (uint32_t t = lane; t < a.k; t += 32) {
+                const bool real = t < cnt[j];
+                const uint64_t key = real ? L[j][t] : kKeyNone;
+                const uint32_t pid = key_pid(key);
+                a.out_ids[qi * a.k + t] = real ? (a.id_map ? a.id_map[pid] : pid) : kInvalid;
+                if (a.out_dist) a.out_dist[qi * a.k + t] = real ? reported_distance(key_dbits(key), a.metric) : __int_as_float(0x7f800000);
+            }
+            if (a.out_len && lane == 0) a.out_len[qi] = cnt[j];
+        } else {  // K4 reads k keys per list
+            for (uint32_t t = cnt[j] + lane; t < a.k; t += 32) L[j][t] = kKeyNone;
+        }
+    }
+}
+
+__global__ void apply_id_map_kernel(uint32_t* ids, uint64_t n, const uint32_t* id_map) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+        if (ids[i] != kInvalid) ids[i] = id_map[ids[i]];
+}
+
+using ScanKernel = void (*)(ExactArgs);
+struct ScanChoice {
+    ScanKernel fn;
+    int qw;
+};
+template <int CH>
+ScanChoice scan_choice(bool bf16) {
+    return ScanChoice{bf16 ? exact_scan_kernel<CH, RowBF16> : exact_scan_kernel<CH, RowF32>, ExactShape<CH>::QW};
+}
+ScanChoice pick_scan(uint32_t nchunks, bool bf16) {
+    switch (kernel_ch(nchunks)) {
+        case 1: return scan_choice<1>(bf16);
+        case 2: return scan_choice<2>(bf16);
+        case 3: return scan_choice<3>(bf16);
+        case 4: return scan_choice<4>(bf16);
+        case 6: return scan_choice<6>(bf16);
+        case 8: return scan_choice<8>(bf16);
+        default: return scan_choice<0>(bf16);
+    }
+}
+
+}  // namespace
+
+// The exact search of nq queries (d_queries: q_stride >= dim floats per row, any alignment, on the index's device) enqueued on the
+// lane's stream.  The caller holds ln.mu.  The lane's diagnostics of approximate searches are left as they are.
+static idb_status enqueue_exact(Index* ix, Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t k, uint32_t* d_ids,
+                                float* d_dist, uint32_t* d_len) {
+    CUDA_TRY(cudaSetDevice(ix->device));
+    cudaStream_t st = ln.stream;
+    if (ix->n == 0) {
+        CUDA_TRY(fill_u32(d_ids, nq * k, kInvalid, st));
+        if (d_dist) CUDA_TRY(fill_u32(reinterpret_cast<uint32_t*>(d_dist), nq * k, 0x7f800000u, st));
+        if (d_len) CUDA_TRY(cudaMemsetAsync(d_len, 0, nq * 4, st));
+        return IDB_OK;
+    }
+    const uint32_t nchunks = ix->nchunks;
+    const size_t stride = (size_t)nchunks * 4;
+    const float* qp = d_queries;
+    if (ix->metric == kMetricCosine) {  // the query normalised once per call, as Index::enqueue_search does it
+        CUDA_TRY(ensure_f32(ln.qn, ln.qn_cap, nq * stride));
+        CUDA_TRY(normalize_rows(d_queries, q_stride, ln.qn, nq, ix->dim, nchunks, ix->num_sms, st));
+        qp = ln.qn;
+    } else if (q_stride != stride || (reinterpret_cast<uintptr_t>(d_queries) & 15)) {
+        CUDA_TRY(ensure_f32(ln.q, ln.q_cap, nq * stride));
+        CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, st));
+        CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, d_queries, q_stride * 4, ix->dim * 4, nq, cudaMemcpyDeviceToDevice, st));
+        qp = ln.q;
+    }
+
+    const ScanChoice sc = pick_scan(nchunks, ix->bf16);
+    int wpc = kExactWarps;
+    size_t smem = 0;
+    if (kernel_ch(nchunks) == 0) {  // one query per warp in shared memory: fewer warps per CTA for very long rows
+        int max_smem = 0;
+        CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ix->device));
+        const size_t per_warp = (size_t)(nchunks + 31) / 32 * 32 * 16;
+        wpc = (int)std::min<size_t>(kExactWarps, (size_t)max_smem / per_warp);
+        if (wpc < 1) return fail(IDB_ERR_UNSUPPORTED, "dim %u: one query does not fit the device's shared memory", ix->dim);
+        smem = per_warp * wpc;
+        if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(sc.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
+    int occ = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sc.fn, wpc * 32, smem));
+    const uint64_t q_per_cta = (uint64_t)wpc * sc.qw;
+
+    // Slices: enough CTAs for about four waves of the device; K4 merges S lists of k keys per query, so S x k stays small, and a
+    // slice keeps at least kExactMinSliceRows rows.  S = 1 (no merge) when the queries alone fill the device.
+    const uint64_t cap_keys = ix->exact_scratch_keys ? ix->exact_scratch_keys : kExactScratchKeys;
+    const uint64_t nq_eff = std::max<uint64_t>(1, std::min<uint64_t>(nq, cap_keys / k));
+    const uint64_t want_ctas = 4ull * std::max(1, occ) * ix->num_sms;
+    const uint64_t q_ctas = (nq_eff + q_per_cta - 1) / q_per_cta;
+    uint64_t S = (want_ctas + q_ctas - 1) / q_ctas;
+    S = std::min<uint64_t>(S, std::max<uint64_t>(1, kExactMaxSliceKeys / k));
+    S = std::min<uint64_t>(S, (ix->n + kExactMinSliceRows - 1) / kExactMinSliceRows);
+    S = std::max<uint64_t>(S, 1);
+    int max_smem = 0;
+    if (S > 1) {
+        idb_status s = merge_fits(ix, S, k, &max_smem);
+        if (s != IDB_OK) return s;
+    }
+    const uint64_t chunk = std::max<uint64_t>(1, cap_keys / (S * k));
+    CUDA_TRY(ensure_u64(ln.exact_keys, ln.exact_keys_cap, S * std::min(nq, chunk) * k));
+
+    ExactArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.g = ix->view();
+    a.k = k;
+    a.S = (uint32_t)S;
+    a.slice_rows = (ix->n + S - 1) / S;
+    a.lists = ln.exact_keys;
+    a.id_map = ix->d_id_map;
+    a.metric = ix->metric;
+    for (uint64_t c0 = 0; c0 < nq; c0 += chunk) {
+        const uint64_t m = std::min(chunk, nq - c0);
+        a.queries = reinterpret_cast<const float4*>(qp + c0 * stride);
+        a.nq = m;
+        a.out_ids = d_ids + c0 * k;
+        a.out_dist = d_dist ? d_dist + c0 * k : nullptr;
+        a.out_len = d_len ? d_len + c0 : nullptr;
+        const dim3 grid((unsigned)((m + q_per_cta - 1) / q_per_cta), (unsigned)S);
+        sc.fn<<<grid, wpc * 32, smem, st>>>(a);
+        CUDA_TRY(cudaGetLastError());
+        if (S > 1) {
+            idb_status s = launch_merge(ix, st, a.lists, (uint32_t)S, m, k, a.out_ids, a.out_dist, a.out_len, nullptr, max_smem);
+            if (s != IDB_OK) return s;
+            if (a.id_map) {  // after the merge: ties are broken by PointId, not by the mapped id
+                const uint64_t cnt = m * k;
+                const unsigned g = (unsigned)std::min<uint64_t>((cnt + 255) / 256, (uint64_t)ix->num_sms * 8);
+                apply_id_map_kernel<<<g, 256, 0, st>>>(a.out_ids, cnt, a.id_map);
+                CUDA_TRY(cudaGetLastError());
+            }
+        }
+    }
+    return IDB_OK;
+}
+
+static idb_status check_exact_args(const void* index, const void* queries, uint64_t nq, const void* out_ids, uint32_t k) {
+    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
+    if (k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
+    if (k > kExactMaxK) return fail(IDB_ERR_UNSUPPORTED, "k = %u > %u is not supported by the exact search", k, kExactMaxK);
+    return IDB_OK;
+}
+
+// A handle exists only where a device does; checked before the handle is touched, so that a call without one fails loudly.
+static idb_status require_device() {
+    int count = 0;
+    cudaError_t e = cudaGetDeviceCount(&count);
+    if (e != cudaSuccess || count == 0)
+        return fail(IDB_ERR_CUDA, "no CUDA device available (%s); this library has no CPU fallback",
+                    e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
+    return IDB_OK;
+}
+
+}  // namespace idb
+
+using namespace idb;
+
+extern "C" {
+
+idb_status idb_exact_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist,
+                                      uint32_t* out_len) {
+    idb_status st = check_exact_args(index, queries, nq, out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
+    if ((st = require_device()) != IDB_OK) return st;
+    Index* ix = reinterpret_cast<Index*>(index);
+    Lane& ln = ix->pick_lane();
+    std::lock_guard<std::mutex> lk(ln.mu, std::adopt_lock);
+    CUDA_TRY(cudaSetDevice(ix->device));
+    CUDA_TRY(ensure_f32(ln.q2, ln.q2_cap, nq * ix->dim));
+    CUDA_TRY(ensure_u32(ln.ids, ln.ids_cap, nq * k));
+    CUDA_TRY(ensure_f32(ln.dist, ln.dist_cap, nq * k));
+    CUDA_TRY(ensure_u32(ln.len, ln.len_cap, nq));
+    CUDA_TRY(cudaMemcpyAsync(ln.q2, queries, nq * ix->dim * 4, cudaMemcpyHostToDevice, ln.stream));
+    st = enqueue_exact(ix, ln, ln.q2, ix->dim, nq, k, ln.ids, ln.dist, ln.len);
+    if (st != IDB_OK) return st;
+    HostOut ho;  // (pageable output buffers are staged through pinned memory: internal.cuh)
+    ho.add(out_ids, ln.ids, nq * k * 4);
+    ho.add(out_dist, ln.dist, nq * k * 4);
+    ho.add(out_len, ln.len, nq * 4);
+    CUDA_TRY(ho.enqueue(ln));
+    CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    ho.finish();
+    return IDB_OK;
+}
+
+idb_status idb_exact_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq, uint32_t k,
+                                              uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len) {
+    idb_status st = check_exact_args(index, d_queries, nq, d_out_ids, k);
+    if (st != IDB_OK) return st;
+    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range (0..%d)", lane, kLanes - 1);
+    if (nq == 0) return IDB_OK;
+    if ((st = require_device()) != IDB_OK) return st;
+    Index* ix = reinterpret_cast<Index*>(index);
+    Lane& ln = ix->lanes[lane];
+    std::lock_guard<std::mutex> lk(ln.mu);
+    return enqueue_exact(ix, ln, d_queries, ix->dim, nq, k, d_out_ids, d_out_dist, d_out_len);
+}
+
+}  // extern "C"

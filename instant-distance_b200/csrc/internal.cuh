@@ -173,6 +173,8 @@ struct Lane {
     uint64_t* keys_all = nullptr;   size_t keys_all_cap = 0;
     float* q2 = nullptr;          size_t q2_cap = 0;
     uint32_t* ids2 = nullptr;     size_t ids2_cap = 0;
+    // exact search: the (query, slice) k-lists of the current query chunk (exact.cu)
+    uint64_t* exact_keys = nullptr; size_t exact_keys_cap = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // host API: results land here first when the caller's output buffers are pageable (see HostOut in api.cu)
     unsigned char* h_out = nullptr; size_t h_out_cap = 0;   // pinned
@@ -245,6 +247,7 @@ struct Index {
     uint32_t b16_cap_16ths = 11;     // IDB_B16_CAP (tests): hand a query to the retry pass beyond this many sixteenths of the slots
     int vis_tier = -1;            // IDB_VIS_TIER: -1 auto (b16 when exact for this n, else bitmap / hash), 0 hash, 1 bitmap, 2 b16
     int variant = 0;              // IDB_VARIANT: alternative (rows in flight, CTAs/SM) instantiations of K1
+    uint64_t exact_scratch_keys = 0;  // IDB_EXACT_SCRATCH_KEYS (tests): keys of an exact call's list scratch per query chunk (0 = default)
     // Adaptive: when more than 1 in 1000 traversals of a call overflowed the b16 tables (data whose traversals visit more ids than
     // the tables were sized for), later calls with that ef or a larger one use the DRAM-resident atomic flavours instead of paying
     // for the retry pass.  Results are identical either way.
@@ -284,6 +287,13 @@ cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
 // dim used, any alignment), one warp per row.  dst may equal src when src_stride == nchunks * 4.
 cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,
                            cudaStream_t st);
+// K4 (merge.cu): per query, the k smallest keys of G lists of k keys (G x nq x k; all ones = empty slot), written as ids / reported
+// distances / lengths, or as keys when d_keys is set.  The merge holds a query's G x k keys per warp in shared memory: merge_fits
+// refuses a merge larger than the device's opt-in shared memory per block and sets *max_smem to that limit, for launch_merge.
+idb_status merge_fits(const Index* ix, uint64_t lists, uint32_t k, int* max_smem);
+idb_status launch_merge(Index* ix, cudaStream_t st, const uint64_t* keys, uint32_t G, uint64_t nq, uint32_t k, uint32_t* d_ids,
+                        float* d_dist, uint32_t* d_len, uint64_t* d_keys, int max_smem);
+
 cudaError_t ensure_u32(uint32_t*& p, size_t& cap, size_t need);
 cudaError_t ensure_u64(uint64_t*& p, size_t& cap, size_t need);
 cudaError_t ensure_f32(float*& p, size_t& cap, size_t need);

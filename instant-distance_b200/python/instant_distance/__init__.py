@@ -6,6 +6,8 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
     here every point of an index is zero-padded to the longest point given at build time, and a longer query raises the
     same `TypeError("point array too long")`, py:369-370);
   * `Hnsw.search_many / HnswMap.search_many` expose the batched search the GPU is built for;
+  * `Hnsw.search_exact / HnswMap.search_exact` return the exact k nearest points (a scan of every point, ties by lower PointId),
+    the ground truth to tune `ef_search` against;
   * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
     DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it.
 """
@@ -119,6 +121,11 @@ class Hnsw:
         """Batched Hnsw::search: returns (ids [nq, k], distances [nq, k], lens [nq])."""
         q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
         return self._ix.search(q, ef_search=ef_search or self._ef, k=k)
+
+    def search_exact(self, points, k=10):
+        """Exact k-NN over every point of the index: returns (ids [nq, k], distances [nq, k], lens [nq]) like search_many."""
+        q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
+        return self._ix.exact_search(q, k=k)
 
     def dump(self, fname):
         """py:131-137: bincode layout of `Hnsw` (ef_search, points, zero, layers)."""

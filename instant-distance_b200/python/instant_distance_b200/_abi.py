@@ -25,6 +25,7 @@ SYMBOLS = [
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
+    "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane",
 ]
 
 
@@ -77,6 +78,8 @@ def lib():
     L.idb_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.c_uint32, u32p, f32p, u32p]
     L.idb_search_batch_device.argtypes = [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, vp]
     L.idb_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, vp]
+    L.idb_exact_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, u32p, f32p, u32p]
+    L.idb_exact_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, vp, vp, vp]
     L.idb_last_search_counters.argtypes = [vp, C.c_uint64, u64p]
     L.idb_last_search_failures.argtypes = [vp, C.c_uint32, u32p]
     L.idb_last_search_retried.argtypes = [vp, C.c_uint32, u32p]
@@ -257,6 +260,21 @@ class Index:
     def search_device(self, d_queries, nq, ef_search, k, d_ids, d_dist, d_len, lane=0):
         """Asynchronous: enqueues on submission lane `lane` (own stream; lanes overlap on the device)."""
         check(lib().idb_search_batch_device_lane(self._h, lane, d_queries, nq, ef_search, k, d_ids, d_dist, d_len))
+
+    def exact_search(self, queries, k=10):
+        """Exact k-NN over every stored row (idb_exact_search_batch_f32): (ids, dist, lens) laid out like search()."""
+        q = self._queries(queries)
+        nq = q.shape[0]
+        ids = np.empty((nq, k), dtype=np.uint32)
+        dist = np.empty((nq, k), dtype=np.float32)
+        lens = np.empty(nq, dtype=np.uint32)
+        check(lib().idb_exact_search_batch_f32(self._h, ptr(q, C.c_float), nq, k, ptr(ids, C.c_uint32), ptr(dist, C.c_float),
+                                               ptr(lens, C.c_uint32)))
+        return ids, dist, lens
+
+    def exact_search_device(self, d_queries, nq, k, d_ids, d_dist, d_len, lane=0):
+        """Asynchronous exact k-NN on device buffers, enqueued on submission lane `lane`."""
+        check(lib().idb_exact_search_batch_device_lane(self._h, lane, d_queries, nq, k, d_ids, d_dist, d_len))
 
     def lane_stream(self, lane):
         return lib().idb_index_lane_stream(self._h, lane)

@@ -36,6 +36,8 @@ extern "C" {
     fn idb_normalize_f32(rows: *const f32, n: u64, dim: u32, device: i32, out: *mut f32) -> i32;
     fn idb_index_metric(ix: *const IdbIndex, out: *mut u32) -> i32;
     fn idb_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, ef: u32, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
+    fn idb_exact_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
+    fn idb_exact_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
     fn idb_index_free(ix: *mut IdbIndex);
     fn idb_last_error() -> *const c_char;
     // Batched / device-side / multi-GPU entry points (no counterpart in the reference; see include/instant_distance_b200.h):
@@ -159,6 +161,14 @@ impl Hnsw {
             search.nearest.extend((0..len as usize).map(|i| (dist[i], PointId(ids[i]))));
         }
         search.nearest.iter().map(move |&(distance, pid)| Item { distance, pid, point: &self.points[pid.0 as usize] })
+    }
+    /// Not in the reference: the exact k nearest points (every point scanned; ties by lower PointId), as (distance, PointId).
+    pub fn search_exact(&self, point: &F32Point, k: usize) -> Vec<(f32, PointId)> {
+        if k == 0 { return Vec::new(); }
+        let (mut ids, mut dist, mut len) = (vec![u32::MAX; k], vec![f32::INFINITY; k], 0u32);
+        let rc = unsafe { idb_exact_search_batch_f32(self.raw, point.0.as_ptr(), 1, k as u32, ids.as_mut_ptr(), dist.as_mut_ptr(), &mut len) };
+        assert_eq!(rc, 0, "{}", last_error());
+        (0..len as usize).map(|i| (dist[i], PointId(ids[i]))).collect()
     }
     pub fn iter(&self) -> impl Iterator<Item = (PointId, &F32Point)> { self.points.iter().enumerate().map(|(i, p)| (PointId(i as u32), p)) }
 }
