@@ -330,41 +330,79 @@ static bool host_ptr_is_pinned(const void* p) {
     return at.type == cudaMemoryTypeHost || at.type == cudaMemoryTypeManaged;
 }
 
-cudaError_t HostOut::enqueue(Lane& ln) {
-    lane = &ln;
-    staged = false;
+// Output buffers in pinned (or registered) host memory receive the copies directly.  Pageable buffers do NOT, and neither do the
+// control blocks: a device-to-pageable cudaMemcpyAsync blocks inside the driver until the copy has run (i.e. until this call's K1 has
+// finished) and stalls the launches of other caller threads meanwhile — concurrent callers would never have a second batch queued
+// behind the running one.  Those results are staged in the lane's pinned buffer and copied out after the stream has been synchronised.
+idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len, Lane* const* ctrl_lanes,
+                     uint32_t n_ctrl) {
+    struct Part { void* user; const void* dev; size_t bytes; size_t off; };
+    Part parts[3] = {{out_ids, ln.ids, nq * k * 4, 0}, {out_dist, ln.dist, nq * k * 4, 0}, {out_len, ln.len, nq * 4, 0}};
+    bool staged = false;
     size_t total = 0;
-    for (int i = 0; i < n; ++i) {
-        staged = staged || !host_ptr_is_pinned(parts[i].user);
-        parts[i].off = total;
-        total += (parts[i].bytes + 63) / 64 * 64;
+    for (Part& p : parts) {
+        if (!p.user) continue;
+        staged = staged || !host_ptr_is_pinned(p.user);
+        p.off = total;
+        total += (p.bytes + 63) / 64 * 64;
     }
     if (staged && total > ln.h_out_cap) {
         if (ln.h_out) cudaFreeHost(ln.h_out);
         ln.h_out = nullptr;
         ln.h_out_cap = 0;
-        const size_t want = total + total / 4;
-        cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&ln.h_out), want, cudaHostAllocDefault);
-        if (e != cudaSuccess) return e;
-        ln.h_out_cap = want;
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&ln.h_out), total + total / 4, cudaHostAllocDefault));
+        ln.h_out_cap = total + total / 4;
     }
-    for (int i = 0; i < n; ++i) {
-        void* dst = staged ? static_cast<void*>(ln.h_out + parts[i].off) : parts[i].user;
-        cudaError_t e = cudaMemcpyAsync(dst, parts[i].dev, parts[i].bytes, cudaMemcpyDeviceToHost, ln.stream);
-        if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
+    for (const Part& p : parts)
+        if (p.user)
+            CUDA_TRY(cudaMemcpyAsync(staged ? static_cast<void*>(ln.h_out + p.off) : p.user, p.dev, p.bytes, cudaMemcpyDeviceToHost, ln.stream));
+    for (uint32_t i = 0; i < n_ctrl; ++i)
+        if (ctrl_lanes[i]->last_nq)
+            CUDA_TRY(cudaMemcpyAsync(ctrl_lanes[i]->h_ctrl + 1, ctrl_lanes[i]->ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
+    CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    for (const Part& p : parts)
+        if (staged && p.user) std::memcpy(p.user, ln.h_out + p.off, p.bytes);
+    uint64_t failed = 0;  // failures that survived the retry pass
+    for (uint32_t i = 0; i < n_ctrl; ++i)
+        if (ctrl_lanes[i]->last_nq) failed += ctrl_lanes[i]->h_ctrl[1].retry.fail_count;
+    if (failed)
+        return fail(IDB_ERR_CAPACITY, "%llu traversals of %llu queries overflowed an internal per-query structure (visited table / tie list)",
+                    (unsigned long long)failed, (unsigned long long)nq);
+    return IDB_OK;
 }
 
-void HostOut::finish() const {
-    if (!staged) return;
-    for (int i = 0; i < n; ++i) std::memcpy(parts[i].user, lane->h_out + parts[i].off, parts[i].bytes);
+idb_status require_device(int* count) {
+    int c = 0;
+    cudaError_t e = cudaGetDeviceCount(&c);
+    if (e != cudaSuccess || c == 0)
+        return fail(IDB_ERR_CUDA, "no CUDA device available (%s); this library has no CPU fallback",
+                    e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
+    if (count) *count = c;
+    return IDB_OK;
+}
+
+idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shards, const void* comm, const uint32_t* lane,
+                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k) {
+    if (f == Family::sharded && !comm) return fail(IDB_ERR_INVALID_ARG, "comm is null");
+    if (f != Family::sharded && !shards[0]) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
+    if ((nq > 0 || f == Family::exact) && k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
+    if (f == Family::exact && k > kExactMaxK)
+        return fail(IDB_ERR_UNSUPPORTED, "k = %u > %u is not supported by the exact search", k, kExactMaxK);
+    if (lane && *lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range (0..%d)", *lane, kLanes - 1);
+    if (nq == 0) return IDB_OK;
+    if (f == Family::sharded) {
+        if (!shards || n_shards == 0 || n_shards > 64) return fail(IDB_ERR_INVALID_ARG, "shards: need 1..64 index handles");
+        for (uint32_t i = 0; i < n_shards; ++i)
+            if (!shards[i]) return fail(IDB_ERR_INVALID_ARG, "shard %u is null", i);
+    }
+    return require_device();
 }
 
 void Lane::free_all() {
     cudaFree(ctrl); cudaFree(status); cudaFree(fail_list); cudaFree(counters);
     cudaFree(q); cudaFree(qn); cudaFree(ids); cudaFree(dist); cudaFree(len);
-    cudaFree(keys_local); cudaFree(keys_all); cudaFree(q2); cudaFree(ids2); cudaFree(exact_keys);
+    cudaFree(keys_local); cudaFree(keys_all); cudaFree(shard_ids); cudaFree(exact_keys);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (ev_ctrl) cudaEventDestroy(ev_ctrl);
@@ -518,9 +556,57 @@ idb_status Index::select_visited_tier(uint32_t ef, VisTier& t, LaunchWindow& win
 
 int Index::search_grid() const { return num_sms * ctx->slots_per_sm; }
 
+cudaError_t write_empty(cudaStream_t st, uint64_t nq, uint32_t k, uint32_t* ids, float* dist, uint32_t* len, uint64_t* keys) {
+    cudaError_t e = fill_u32(ids, nq * k, kInvalid, st);
+    if (e == cudaSuccess && dist) e = fill_u32(reinterpret_cast<uint32_t*>(dist), nq * k, 0x7f800000u, st);
+    if (e == cudaSuccess && len) e = cudaMemsetAsync(len, 0, nq * 4, st);
+    if (e == cudaSuccess && keys) e = cudaMemsetAsync(keys, 0xFF, nq * k * 8, st);  // kKeyNone everywhere
+    return e;
+}
+
+idb_status Index::stage_queries(Lane& ln, const float* queries, bool host, uint64_t nq, const float** out) {
+    const size_t stride = (size_t)nchunks * 4;
+    *out = queries;
+    if (!host && stride == dim && !(reinterpret_cast<uintptr_t>(queries) & 15)) return IDB_OK;
+    CUDA_TRY(ensure(ln.q, ln.q_cap, nq * stride));
+    const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    if (stride == dim) {
+        CUDA_TRY(cudaMemcpyAsync(ln.q, queries, nq * stride * 4, kind, ln.stream));
+    } else {
+        CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, ln.stream));
+        CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, queries, dim * 4, dim * 4, nq, kind, ln.stream));
+    }
+    *out = ln.q;
+    return IDB_OK;
+}
+
+idb_status Index::normalize_queries(Lane& ln, const float** q, uint64_t nq) {
+    if (metric != kMetricCosine) return IDB_OK;
+    CUDA_TRY(ensure(ln.qn, ln.qn_cap, nq * nchunks * 4));
+    CUDA_TRY(normalize_rows(*q, (uint64_t)nchunks * 4, ln.qn, nq, dim, nchunks, num_sms, ln.stream));
+    *q = ln.qn;
+    return IDB_OK;
+}
+
+idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged, uint64_t nq, uint32_t ef_search, uint32_t k,
+                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys) {
+    CUDA_TRY(cudaSetDevice(ix->device));
+    const uint32_t ef = ef_search ? ef_search : ix->ef_search;
+    if (ix->n == 0 || ef == 0) {  // empty index (core:359-361) / ef_search = 0: empty result lists
+        CUDA_TRY(write_empty(ln.stream, nq, k, d_ids, d_dist, d_len, d_keys));
+        ln.last_nq = 0;
+        return IDB_OK;
+    }
+    if (!staged) {
+        idb_status st = ix->stage_queries(ln, queries, false, nq, &queries);
+        if (st != IDB_OK) return st;
+    }
+    return ix->enqueue_search(ln, queries, nq, ef, k, d_ids, d_dist, d_len, d_keys);
+}
+
 // Enqueue one batched search on a lane; all pointers are device pointers (d_queries: see internal.cuh).  The caller holds ln.mu.
-idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
-                                 float* d_dist, uint32_t* d_len, uint64_t* out_keys) {
+idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids, float* d_dist,
+                                 uint32_t* d_len, uint64_t* out_keys) {
     if (n) ef = (uint32_t)std::min<uint64_t>(ef, n);  // admission is rank < ef and there are only n distinct ids: same results
     if (ef > 1024) return fail(IDB_ERR_UNSUPPORTED, "ef_search %u > 1024 (on an index of more than 1024 points) is not supported", ef);
     idb_status st = ensure_lane_scratch(ln, nq);
@@ -530,7 +616,6 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     SearchArgs a;
     std::memset(&a, 0, sizeof(a));
     a.g = view();
-    a.queries = reinterpret_cast<const float4*>(d_queries);
     a.metric = metric;
     a.work.n_work = nq;
     a.work.work_counter = &ln.ctrl->main.work_counter;
@@ -555,11 +640,9 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t q_st
     const int row_t = (int)((2 * M + 31) / 32);
     const int ef_t = (int)((ef + 31) / 32);
     const int grid = std::max(1, (int)std::min<uint64_t>((nq + kSearchWarps - 1) / kSearchWarps, (uint64_t)search_grid()));
-    if (metric == kMetricCosine) {  // once per call: K1 and the retry pass read the same normalised rows; the caller's stay untouched
-        CUDA_TRY(ensure(ln.qn, ln.qn_cap, nq * nchunks * 4));
-        CUDA_TRY(normalize_rows(d_queries, q_stride, ln.qn, nq, dim, nchunks, num_sms, ln.stream));
-        a.queries = reinterpret_cast<const float4*>(ln.qn);
-    }
+    st = normalize_queries(ln, &d_queries, nq);  // once per call: K1 and the retry pass read the same rows
+    if (st != IDB_OK) return st;
+    a.queries = reinterpret_cast<const float4*>(d_queries);
 
     std::lock_guard<std::mutex> lk(ctx->mu);  // the tables this launch uses must not be regrown under it
     LaunchWindow win;
@@ -652,10 +735,8 @@ Index::~Index() {
 
 idb_status Index::init_device(int dev) {
     int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0)
-        return fail(IDB_ERR_CUDA, "no CUDA device available (%s); this library has no CPU fallback",
-                    e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
+    idb_status st = require_device(&count);
+    if (st != IDB_OK) return st;
     if (dev < 0 || dev >= count) return fail(IDB_ERR_INVALID_ARG, "device %d out of range (0..%d)", dev, count - 1);
     device = dev;
     CUDA_TRY(cudaSetDevice(dev));
@@ -664,7 +745,7 @@ idb_status Index::init_device(int dev) {
     if (prop.major != 9 || prop.minor != 0)
         return fail(IDB_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", dev, prop.major, prop.minor);
     num_sms = prop.multiProcessorCount;
-    idb_status st = DeviceCtx::acquire(dev, &ctx);
+    st = DeviceCtx::acquire(dev, &ctx);
     if (st != IDB_OK) return st;
     for (auto& ln : lanes) CUDA_TRY(cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking));
     stream = lanes[0].stream;
@@ -844,53 +925,17 @@ idb_status idb_index_from_graph_bf16(const float* points, uint64_t n, uint32_t d
 
 }  // extern "C"
 
-namespace idb {
-static idb_status search_device_on_lane(Index* ix, Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef_search, uint32_t k,
-                                        uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len, uint64_t* out_keys) {
-    CUDA_TRY(cudaSetDevice(ix->device));
-    const uint32_t ef = ef_search ? ef_search : ix->ef_search;
-    if (ix->n == 0 || ef == 0) {  // empty index (core:359-361) / ef_search = 0: empty result lists
-        CUDA_TRY(fill_u32(d_out_ids, nq * k, kInvalid, ln.stream));
-        if (d_out_dist) CUDA_TRY(fill_u32(reinterpret_cast<uint32_t*>(d_out_dist), nq * k, 0x7f800000u, ln.stream));
-        if (d_out_len) CUDA_TRY(cudaMemsetAsync(d_out_len, 0, nq * 4, ln.stream));
-        if (out_keys) CUDA_TRY(cudaMemsetAsync(out_keys, 0xFF, nq * k * 8, ln.stream));  // kKeyNone everywhere
-        ln.last_nq = 0;
-        return IDB_OK;
-    }
-    if (ix->metric == kMetricCosine)  // the normalisation writes padded rows itself
-        return ix->enqueue_search(ln, d_queries, ix->dim, nq, ef, k, d_out_ids, d_out_dist, d_out_len, out_keys);
-    const float* qp = d_queries;
-    const size_t stride = (size_t)ix->nchunks * 4;
-    if (stride != ix->dim || (reinterpret_cast<uintptr_t>(d_queries) & 15)) {
-        CUDA_TRY(ensure(ln.q, ln.q_cap, nq * stride));
-        CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, ln.stream));
-        CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, d_queries, ix->dim * 4, ix->dim * 4, nq, cudaMemcpyDeviceToDevice, ln.stream));
-        qp = ln.q;
-    }
-    return ix->enqueue_search(ln, qp, stride, nq, ef, k, d_out_ids, d_out_dist, d_out_len, out_keys);
-}
-
-// used by sharded.cu: lane 0, caller holds its mutex
-idb_status search_device_keys(Index* ix, Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef_search, uint32_t k, uint32_t* d_ids,
-                              uint64_t* d_keys) {
-    return search_device_on_lane(ix, ln, d_queries, nq, ef_search, k, d_ids, nullptr, nullptr, d_keys);
-}
-}  // namespace idb
-
 extern "C" {
 
 idb_status idb_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq, uint32_t ef_search,
                                         uint32_t k, uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len) {
-    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    idb_status st = check_search_args(Family::approx, &index, 1, nullptr, &lane, d_queries, nq, d_out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
     Index* ix = reinterpret_cast<Index*>(index);
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range (0..%d)", lane, kLanes - 1);
-    if (nq == 0) return IDB_OK;
-    if (!d_queries || !d_out_ids) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
-    if (k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
     Lane& ln = ix->lanes[lane];
     std::lock_guard<std::mutex> lk(ln.mu);
     ix->last_lane.store((int)lane);
-    return search_device_on_lane(ix, ln, d_queries, nq, ef_search, k, d_out_ids, d_out_dist, d_out_len, nullptr);
+    return search_on_lane(ix, ln, d_queries, false, nq, ef_search, k, d_out_ids, d_out_dist, d_out_len, nullptr);
 }
 
 idb_status idb_search_batch_device(idb_index* index, const float* d_queries, uint64_t nq, uint32_t ef_search, uint32_t k,
@@ -900,11 +945,9 @@ idb_status idb_search_batch_device(idb_index* index, const float* d_queries, uin
 
 idb_status idb_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, uint32_t ef_search, uint32_t k,
                                 uint32_t* out_ids, float* out_dist, uint32_t* out_len) {
-    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    idb_status st = check_search_args(Family::approx, &index, 1, nullptr, nullptr, queries, nq, out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
     Index* ix = reinterpret_cast<Index*>(index);
-    if (nq == 0) return IDB_OK;
-    if (!queries || !out_ids) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
-    if (k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
     const uint32_t ef = ef_search ? ef_search : ix->ef_search;
     if (ix->n == 0 || ef == 0) {
         for (uint64_t i = 0; i < nq * k; ++i) out_ids[i] = IDB_INVALID;
@@ -918,38 +961,17 @@ idb_status idb_search_batch_f32(idb_index* index, const float* queries, uint64_t
     std::lock_guard<std::mutex> lk(ln.mu, std::adopt_lock);
     ix->last_lane.store((int)(&ln - ix->lanes));
     CUDA_TRY(cudaSetDevice(ix->device));
-    const size_t stride = (size_t)ix->nchunks * 4;
-    CUDA_TRY(ensure(ln.q, ln.q_cap, nq * stride));
     CUDA_TRY(ensure(ln.ids, ln.ids_cap, nq * k));
     CUDA_TRY(ensure(ln.dist, ln.dist_cap, nq * k));
     CUDA_TRY(ensure(ln.len, ln.len_cap, nq));
-    uint64_t q_stride = stride;
-    if (stride == ix->dim || ix->metric == kMetricCosine) {  // (cosine: the normalisation writes padded rows itself)
-        CUDA_TRY(cudaMemcpyAsync(ln.q, queries, nq * ix->dim * 4, cudaMemcpyHostToDevice, ln.stream));
-        q_stride = ix->dim;
-    } else {
-        CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, ln.stream));
-        CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, queries, ix->dim * 4, ix->dim * 4, nq, cudaMemcpyHostToDevice, ln.stream));
-    }
-    idb_status st = ix->enqueue_search(ln, ln.q, q_stride, nq, ef, k, ln.ids, ln.dist, ln.len, nullptr);
+    const float* qp = nullptr;
+    st = ix->stage_queries(ln, queries, true, nq, &qp);
+    if (st == IDB_OK) st = ix->enqueue_search(ln, qp, nq, ef, k, ln.ids, ln.dist, ln.len, nullptr);
     if (st != IDB_OK) return st;
-    HostOut ho;
-    ho.add(out_ids, ln.ids, nq * k * 4);
-    ho.add(out_dist, ln.dist, nq * k * 4);
-    ho.add(out_len, ln.len, nq * 4);
-    CUDA_TRY(ho.enqueue(ln));
-    // The control block comes back through PINNED memory: a device-to-pageable cudaMemcpyAsync blocks inside the driver until the
-    // copy has run (i.e. until this call's K1 has finished) and stalls the launches of other caller threads meanwhile, so concurrent
-    // callers would never have a second batch queued behind the running one.
-    const SearchCtrl& ctrl = ln.h_ctrl[1];
-    CUDA_TRY(cudaMemcpyAsync(ln.h_ctrl + 1, ln.ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    ho.finish();
-    ix->note_overflows(ef, nq, ctrl.main.fail_count, ln.last_b16);
-    if (ctrl.retry.fail_count != 0)  // failures that survived the retry pass
-        return fail(IDB_ERR_CAPACITY, "%u of %llu queries overflowed an internal per-query structure (visited table / tie list)",
-                    ctrl.retry.fail_count, (unsigned long long)nq);
-    return IDB_OK;
+    Lane* lp = &ln;
+    st = read_back(ln, nq, k, out_ids, out_dist, out_len, &lp, 1);
+    if (st == IDB_OK || st == IDB_ERR_CAPACITY) ix->note_overflows(ef, nq, ln.h_ctrl[1].main.fail_count, ln.last_b16);
+    return st;
 }
 
 idb_status idb_last_search_failures(idb_index* index, uint32_t lane, uint32_t* out_failed) {
@@ -1092,9 +1114,8 @@ void idb_index_free(idb_index* index) { delete reinterpret_cast<Index*>(index); 
 
 idb_status idb_distance_f32(const float* a, const float* b, uint32_t dim, int32_t device, float* out) {
     if (!a || !b || !out || dim == 0) return fail(IDB_ERR_INVALID_ARG, "null argument or dim == 0");
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-        return fail(IDB_ERR_CUDA, "no CUDA device available; this library has no CPU fallback");
+    idb_status st = require_device();
+    if (st != IDB_OK) return st;
     CUDA_TRY(cudaSetDevice(device));
     const uint32_t nchunks = (dim + 3) / 4;
     float* d = nullptr;
@@ -1113,8 +1134,8 @@ idb_status idb_distance_f32(const float* a, const float* b, uint32_t dim, int32_
 idb_status idb_normalize_f32(const float* rows, uint64_t n, uint32_t dim, int32_t device, float* out) {
     if (dim == 0 || (n && (!rows || !out))) return fail(IDB_ERR_INVALID_ARG, "null argument or dim == 0");
     int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0)
-        return fail(IDB_ERR_CUDA, "no CUDA device available; this library has no CPU fallback");
+    idb_status st = require_device(&count);
+    if (st != IDB_OK) return st;
     if (device < 0 || device >= count) return fail(IDB_ERR_INVALID_ARG, "device %d out of range (0..%d)", device, count - 1);
     if (n == 0) return IDB_OK;
     CUDA_TRY(cudaSetDevice(device));

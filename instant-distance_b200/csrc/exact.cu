@@ -15,7 +15,6 @@ namespace idb {
 
 namespace {
 
-constexpr uint32_t kExactMaxK = 1024;
 constexpr int kExactWarps = 8;                 // warps per CTA: they walk the same rows in the same order (L1 serves the others)
 constexpr uint64_t kExactScratchKeys = 1ull << 25;  // keys of per-call list scratch (256 MB): larger batches run in query chunks
 constexpr uint32_t kExactMaxSliceKeys = 2048;  // slices x k: K4's cost grows with its square
@@ -209,31 +208,22 @@ ScanChoice pick_scan(uint32_t nchunks, bool bf16) {
 
 }  // namespace
 
-// The exact search of nq queries (d_queries: q_stride >= dim floats per row, any alignment, on the index's device) enqueued on the
-// lane's stream.  The caller holds ln.mu.  The lane's diagnostics of approximate searches are left as they are.
-static idb_status enqueue_exact(Index* ix, Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t k, uint32_t* d_ids,
+// The exact search of nq queries (dim floats per row, any alignment, in host memory when `host`, else on the index's device)
+// enqueued on the lane's stream.  The caller holds ln.mu.  The lane's diagnostics of approximate searches are left as they are.
+static idb_status enqueue_exact(Index* ix, Lane& ln, const float* queries, bool host, uint64_t nq, uint32_t k, uint32_t* d_ids,
                                 float* d_dist, uint32_t* d_len) {
     CUDA_TRY(cudaSetDevice(ix->device));
     cudaStream_t st = ln.stream;
     if (ix->n == 0) {
-        CUDA_TRY(fill_u32(d_ids, nq * k, kInvalid, st));
-        if (d_dist) CUDA_TRY(fill_u32(reinterpret_cast<uint32_t*>(d_dist), nq * k, 0x7f800000u, st));
-        if (d_len) CUDA_TRY(cudaMemsetAsync(d_len, 0, nq * 4, st));
+        CUDA_TRY(write_empty(st, nq, k, d_ids, d_dist, d_len, nullptr));
         return IDB_OK;
     }
     const uint32_t nchunks = ix->nchunks;
     const size_t stride = (size_t)nchunks * 4;
-    const float* qp = d_queries;
-    if (ix->metric == kMetricCosine) {  // the query normalised once per call, as Index::enqueue_search does it
-        CUDA_TRY(ensure_f32(ln.qn, ln.qn_cap, nq * stride));
-        CUDA_TRY(normalize_rows(d_queries, q_stride, ln.qn, nq, ix->dim, nchunks, ix->num_sms, st));
-        qp = ln.qn;
-    } else if (q_stride != stride || (reinterpret_cast<uintptr_t>(d_queries) & 15)) {
-        CUDA_TRY(ensure_f32(ln.q, ln.q_cap, nq * stride));
-        CUDA_TRY(cudaMemsetAsync(ln.q, 0, nq * stride * 4, st));
-        CUDA_TRY(cudaMemcpy2DAsync(ln.q, stride * 4, d_queries, q_stride * 4, ix->dim * 4, nq, cudaMemcpyDeviceToDevice, st));
-        qp = ln.q;
-    }
+    const float* qp = nullptr;
+    idb_status s = ix->stage_queries(ln, queries, host, nq, &qp);
+    if (s == IDB_OK) s = ix->normalize_queries(ln, &qp, nq);
+    if (s != IDB_OK) return s;
 
     const ScanChoice sc = pick_scan(nchunks, ix->bf16);
     int wpc = kExactWarps;
@@ -263,7 +253,7 @@ static idb_status enqueue_exact(Index* ix, Lane& ln, const float* d_queries, uin
     S = std::max<uint64_t>(S, 1);
     int max_smem = 0;
     if (S > 1) {
-        idb_status s = merge_fits(ix, S, k, &max_smem);
+        s = merge_fits(ix, S, k, &max_smem);
         if (s != IDB_OK) return s;
     }
     const uint64_t chunk = std::max<uint64_t>(1, cap_keys / (S * k));
@@ -289,7 +279,7 @@ static idb_status enqueue_exact(Index* ix, Lane& ln, const float* d_queries, uin
         sc.fn<<<grid, wpc * 32, smem, st>>>(a);
         CUDA_TRY(cudaGetLastError());
         if (S > 1) {
-            idb_status s = launch_merge(ix, st, a.lists, (uint32_t)S, m, k, a.out_ids, a.out_dist, a.out_len, nullptr, max_smem);
+            s = launch_merge(ix, st, a.lists, (uint32_t)S, m, k, a.out_ids, a.out_dist, a.out_len, nullptr, max_smem);
             if (s != IDB_OK) return s;
             if (a.id_map) {  // after the merge: ties are broken by PointId, not by the mapped id
                 const uint64_t cnt = m * k;
@@ -302,24 +292,6 @@ static idb_status enqueue_exact(Index* ix, Lane& ln, const float* d_queries, uin
     return IDB_OK;
 }
 
-static idb_status check_exact_args(const void* index, const void* queries, uint64_t nq, const void* out_ids, uint32_t k) {
-    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
-    if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
-    if (k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
-    if (k > kExactMaxK) return fail(IDB_ERR_UNSUPPORTED, "k = %u > %u is not supported by the exact search", k, kExactMaxK);
-    return IDB_OK;
-}
-
-// A handle exists only where a device does; checked before the handle is touched, so that a call without one fails loudly.
-static idb_status require_device() {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0)
-        return fail(IDB_ERR_CUDA, "no CUDA device available (%s); this library has no CPU fallback",
-                    e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
-    return IDB_OK;
-}
-
 }  // namespace idb
 
 using namespace idb;
@@ -328,41 +300,28 @@ extern "C" {
 
 idb_status idb_exact_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist,
                                       uint32_t* out_len) {
-    idb_status st = check_exact_args(index, queries, nq, out_ids, k);
+    idb_status st = check_search_args(Family::exact, &index, 1, nullptr, nullptr, queries, nq, out_ids, k);
     if (st != IDB_OK || nq == 0) return st;
-    if ((st = require_device()) != IDB_OK) return st;
     Index* ix = reinterpret_cast<Index*>(index);
     Lane& ln = ix->pick_lane();
     std::lock_guard<std::mutex> lk(ln.mu, std::adopt_lock);
     CUDA_TRY(cudaSetDevice(ix->device));
-    CUDA_TRY(ensure_f32(ln.q2, ln.q2_cap, nq * ix->dim));
     CUDA_TRY(ensure_u32(ln.ids, ln.ids_cap, nq * k));
     CUDA_TRY(ensure_f32(ln.dist, ln.dist_cap, nq * k));
     CUDA_TRY(ensure_u32(ln.len, ln.len_cap, nq));
-    CUDA_TRY(cudaMemcpyAsync(ln.q2, queries, nq * ix->dim * 4, cudaMemcpyHostToDevice, ln.stream));
-    st = enqueue_exact(ix, ln, ln.q2, ix->dim, nq, k, ln.ids, ln.dist, ln.len);
+    st = enqueue_exact(ix, ln, queries, true, nq, k, ln.ids, ln.dist, ln.len);
     if (st != IDB_OK) return st;
-    HostOut ho;  // (pageable output buffers are staged through pinned memory: internal.cuh)
-    ho.add(out_ids, ln.ids, nq * k * 4);
-    ho.add(out_dist, ln.dist, nq * k * 4);
-    ho.add(out_len, ln.len, nq * 4);
-    CUDA_TRY(ho.enqueue(ln));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    ho.finish();
-    return IDB_OK;
+    return read_back(ln, nq, k, out_ids, out_dist, out_len, nullptr, 0);
 }
 
 idb_status idb_exact_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq, uint32_t k,
                                               uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len) {
-    idb_status st = check_exact_args(index, d_queries, nq, d_out_ids, k);
-    if (st != IDB_OK) return st;
-    if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range (0..%d)", lane, kLanes - 1);
-    if (nq == 0) return IDB_OK;
-    if ((st = require_device()) != IDB_OK) return st;
+    idb_status st = check_search_args(Family::exact, &index, 1, nullptr, &lane, d_queries, nq, d_out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
     Index* ix = reinterpret_cast<Index*>(index);
     Lane& ln = ix->lanes[lane];
     std::lock_guard<std::mutex> lk(ln.mu);
-    return enqueue_exact(ix, ln, d_queries, ix->dim, nq, k, d_out_ids, d_out_dist, d_out_len);
+    return enqueue_exact(ix, ln, d_queries, false, nq, k, d_out_ids, d_out_dist, d_out_len);
 }
 
 }  // extern "C"

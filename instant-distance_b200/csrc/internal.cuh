@@ -163,23 +163,22 @@ struct Lane {
     uint32_t* status = nullptr;   size_t status_cap = 0;
     uint32_t* fail_list = nullptr; size_t fail_cap = 0;
     uint32_t* counters = nullptr; size_t counters_cap = 0;
-    float* q = nullptr;           size_t q_cap = 0;
-    float* qn = nullptr;          size_t qn_cap = 0;   // a cosine call's normalised queries (K1 and its retry pass read them)
+    float* q = nullptr;           size_t q_cap = 0;    // the call's queries in the kernel layout (Index::stage_queries)
+    float* qn = nullptr;          size_t qn_cap = 0;   // a cosine call's normalised queries (Index::normalize_queries)
     uint32_t* ids = nullptr;      size_t ids_cap = 0;
     float* dist = nullptr;        size_t dist_cap = 0;
     uint32_t* len = nullptr;      size_t len_cap = 0;
     // sharded search
     uint64_t* keys_local = nullptr; size_t keys_local_cap = 0;
     uint64_t* keys_all = nullptr;   size_t keys_all_cap = 0;
-    float* q2 = nullptr;          size_t q2_cap = 0;
-    uint32_t* ids2 = nullptr;     size_t ids2_cap = 0;
+    uint32_t* shard_ids = nullptr;  size_t shard_ids_cap = 0;   // the shard's K1 ids (its keys carry the results)
     // exact search: the (query, slice) k-lists of the current query chunk (exact.cu)
     uint64_t* exact_keys = nullptr; size_t exact_keys_cap = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    // host API: results land here first when the caller's output buffers are pageable (see HostOut in api.cu)
+    // host API: results land here first when the caller's output buffers are pageable (see read_back in api.cu)
     unsigned char* h_out = nullptr; size_t h_out_cap = 0;   // pinned
     // asynchronous read-back of the control block of the lane's last call (how many queries overflowed the b16 tables)
-    SearchCtrl* h_ctrl = nullptr;    // pinned, 2 blocks: [0] the sampled overflow tally, [1] the host API's read-back
+    SearchCtrl* h_ctrl = nullptr;    // pinned, 2 blocks: [0] the sampled overflow tally, [1] the host API's read-back (read_back)
     cudaEvent_t ev_ctrl = nullptr;
     bool ctrl_pending = false;
     int ctrl_b16 = 0;
@@ -193,22 +192,6 @@ struct Lane {
     // the template arguments of the lane's last main K1 launch: {CH, ROW_T, EF_T, B, bf16 rows, FULL, TMA, IDB_VARIANT taken}
     uint32_t last_kernel[8] = {};
     void free_all();
-};
-
-// Device -> host copy of a batch's results through the lane's stream.  Output buffers in pinned (or registered) host memory receive
-// the copies directly.  Pageable buffers do NOT: a device-to-pageable cudaMemcpyAsync blocks inside the driver until the copy has run
-// (i.e. until this call's K1 has finished) and stalls the launches of other caller threads meanwhile — concurrent callers would never
-// have a second batch queued behind the running one.  Those results are staged in the lane's pinned buffer and copied out after the
-// stream has been synchronised.
-struct HostOut {
-    struct Part { void* user; const void* dev; size_t bytes; size_t off; };
-    Part parts[3];
-    int n = 0;
-    bool staged = false;
-    Lane* lane = nullptr;
-    void add(void* user, const void* dev, size_t bytes) { if (user && bytes) parts[n++] = Part{user, dev, bytes, 0}; }
-    cudaError_t enqueue(Lane& ln);   // after the kernels of the call
-    void finish() const;             // after cudaStreamSynchronize
 };
 
 struct Index {
@@ -271,16 +254,48 @@ struct Index {
     // because profilers that replay a kernel (ncu) re-launch it without its launch attributes.
     idb_status attach_window(Lane& ln, const LaunchWindow& win);
     idb_status ensure_lane_scratch(Lane& ln, uint64_t nq);
-    // d_queries: q_stride floats per row.  An L2 index takes them as K1 reads them (q_stride = nchunks * 4, zero padded, 16-byte
-    // aligned); a cosine index normalises them into the lane's buffer first (any q_stride >= dim, any alignment).
-    idb_status enqueue_search(Lane& ln, const float* d_queries, uint64_t q_stride, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids,
-                              float* d_dist, uint32_t* d_len, uint64_t* out_keys);
+    // The caller's queries (dim floats per row, in host memory when `host`, else on the device) as the rows K1 and the exact scan
+    // read: nchunks * 4 floats per row, zero padded, 16-byte aligned.  Device rows already laid out so are read where they are;
+    // all others are copied into ln.q in one copy.  *out: the staged rows.
+    idb_status stage_queries(Lane& ln, const float* queries, bool host, uint64_t nq, const float** out);
+    // A cosine index normalises the staged rows *q once per call into ln.qn and points *q there; an L2 index reads them as staged.
+    idb_status normalize_queries(Lane& ln, const float** q, uint64_t nq);
+    // d_queries: staged rows (stage_queries).
+    idb_status enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids, float* d_dist,
+                              uint32_t* d_len, uint64_t* out_keys);
     Lane& pick_lane();
     // For the idb_last_search_* queries: under the lane's lock, what the lane's last search left behind — its control block (`ctrl`,
     // once the lane's stream has drained) and its K1 instantiation (`kernel`, 8 words) — each optional, all zero when the lane has
     // run none.  `latest`: lane 0xFFFFFFFF names the lane of the last call issued on this index.
     idb_status last_search(uint32_t lane, bool latest, SearchCtrl* ctrl, uint32_t* kernel);
 };
+
+constexpr uint32_t kExactMaxK = 1024;  // the exact search's largest k
+
+// Fails with IDB_ERR_CUDA when the runtime sees no device (this library has no CPU fallback); else sets *count if given.
+idb_status require_device(int* count = nullptr);
+
+// The argument checks of a search entry, then require_device.  What differs between the entries: `exact` refuses k = 0 even when
+// nq = 0 and caps k at kExactMaxK; `lane` (optional) must name a lane, even when nq = 0; `sharded` checks comm before anything else
+// and the list of n_shards handles only when nq > 0 (the others check their one handle first).  nq = 0 passes once the checks that
+// apply to it have, without the device check: there is nothing to do.
+enum class Family { approx, exact, sharded };
+idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shards, const void* comm, const uint32_t* lane,
+                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k);
+
+// Empty result lists on the stream: ids INVALID, distances +inf, lengths 0, keys kKeyNone (each output optional but ids).
+cudaError_t write_empty(cudaStream_t st, uint64_t nq, uint32_t k, uint32_t* ids, float* dist, uint32_t* len, uint64_t* keys);
+
+// One approximate search on a lane (the caller holds ln.mu) of staged queries (`staged`) or of the caller's device queries (dim
+// floats per row, any alignment); empty result lists for an empty index or ef_search = 0.
+idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged, uint64_t nq, uint32_t ef_search, uint32_t k,
+                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys);
+
+// The end of a host call on lane ln: copies its results (ln.ids / dist / len, nq x k) to the caller's buffers (each but out_ids
+// optional), reads the control block of each of `ctrl_lanes` whose last call ran K1 into its pinned h_ctrl[1], synchronises the
+// stream, and fails with IDB_ERR_CAPACITY when queries overflowed even the retry pass of those calls.
+idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len, Lane* const* ctrl_lanes,
+                     uint32_t n_ctrl);
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
 // normalize_rows_kernel: dst[r] (nchunks * 4 floats, zero padded) = the canonical normalisation of src[r] (src_stride floats per row,

@@ -126,14 +126,11 @@ idb_status idb_index_set_id_map(idb_index* index, const uint32_t* global_ids) {
 }  // extern "C" (reopened below)
 
 namespace idb {
-idb_status search_device_keys(Index* ix, Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef_search, uint32_t k, uint32_t* d_ids,
-                              uint64_t* d_keys);  // api.cu
-
 // The rank's shards each run K1 on their own lane-0 stream (K1's epilogue packs (distance bits, global id) keys; the launches overlap
 // on the device: one table pool, the next shard's thread blocks move in as the previous shard's drain) -> local pre-merge when the
-// rank holds more than one shard -> ONE ncclAllGather -> merge kernel.  Main stream = lane 0 of the first shard.
-// The caller holds lanes[0].mu of every shard.
-static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, Comm* c, const float* d_queries, uint64_t nq,
+// rank holds more than one shard -> ONE ncclAllGather -> merge kernel.  Main stream = lane 0 of the first shard, which stages the
+// queries (in host memory when `host`, else on the device) once for every shard.  The caller holds lanes[0].mu of every shard.
+static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, Comm* c, const float* queries, bool host, uint64_t nq,
                                         uint32_t ef_search, uint32_t k, uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len) {
     Index* ix = shards[0];
     Lane& ln = ix->lanes[0];
@@ -146,17 +143,20 @@ static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, 
     CUDA_TRY(ensure_u64(ln.keys_local, ln.keys_local_cap, per * (n_local > 1 ? n_local + 1 : 1)));
     CUDA_TRY(ensure_u64(ln.keys_all, ln.keys_all_cap, per * c->world));
     uint64_t* shard_keys = n_local > 1 ? ln.keys_local + per : ln.keys_local;  // [n_local][nq][k]; the pre-merge writes keys_local[0..per)
+    const float* qp = nullptr;
+    st = ix->stage_queries(ln, queries, host, nq, &qp);
+    if (st != IDB_OK) return st;
     cudaEvent_t fork = nullptr;
     if (n_local > 1) {
         CUDA_TRY(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventRecord(fork, ln.stream));  // the queries (and anything else the caller enqueued) are ready
+        CUDA_TRY(cudaEventRecord(fork, ln.stream));  // the staged queries (and anything else the caller enqueued) are ready
     }
     for (uint32_t i = 0; i < n_local && st == IDB_OK; ++i) {
         Index* sx = shards[i];
         Lane& sl = sx->lanes[0];
         if (i > 0 && cudaStreamWaitEvent(sl.stream, fork, 0) != cudaSuccess) st = fail(IDB_ERR_CUDA, "cudaStreamWaitEvent failed");
-        if (st == IDB_OK && cudaSuccess != ensure_u32(sl.ids, sl.ids_cap, per)) st = fail(IDB_ERR_OOM, "scratch allocation failed");
-        if (st == IDB_OK) st = search_device_keys(sx, sl, d_queries, nq, ef_search, k, sl.ids, shard_keys + (size_t)i * per);
+        if (st == IDB_OK && ensure_u32(sl.shard_ids, sl.shard_ids_cap, per) != cudaSuccess) st = fail(IDB_ERR_OOM, "scratch allocation failed");
+        if (st == IDB_OK) st = search_on_lane(sx, sl, qp, true, nq, ef_search, k, sl.shard_ids, nullptr, nullptr, shard_keys + (size_t)i * per);
         if (st == IDB_OK && i > 0) {  // join: the main stream continues after this shard's K1
             cudaEvent_t done = nullptr;
             if (cudaEventCreateWithFlags(&done, cudaEventDisableTiming) != cudaSuccess || cudaEventRecord(done, sl.stream) != cudaSuccess ||
@@ -179,16 +179,15 @@ static idb_status sharded_search_locked(Index* const* shards, uint32_t n_local, 
     return IDB_OK;
 }
 
-// Validates the shard list and locks lane 0 of every shard (in address order: two callers with the same shards cannot deadlock).
+// Checks that the shards (non-null: check_search_args) fit together and locks lane 0 of every shard (in address order: two callers
+// with the same shards cannot deadlock).
 struct ShardLocks {
     std::vector<Index*> order;
     ~ShardLocks() { for (auto it = order.rbegin(); it != order.rend(); ++it) (*it)->lanes[0].mu.unlock(); }
     idb_status lock(idb_index* const* shards, uint32_t n) {
-        if (!shards || n == 0 || n > 64) return fail(IDB_ERR_INVALID_ARG, "shards: need 1..64 index handles");
         std::vector<Index*> v;
         for (uint32_t i = 0; i < n; ++i) {
             Index* ix = reinterpret_cast<Index*>(shards[i]);
-            if (!ix) return fail(IDB_ERR_INVALID_ARG, "shard %u is null", i);
             const Index* first = reinterpret_cast<Index*>(shards[0]);
             if (ix->device != first->device || ix->dim != first->dim)
                 return fail(IDB_ERR_INVALID_ARG, "shard %u: all shards of a rank must live on one device and have one dim", i);
@@ -210,14 +209,12 @@ extern "C" {
 idb_status idb_sharded_search_batch_device_multi(idb_index* const* shards, uint32_t n_shards, idb_comm* comm, const float* d_queries,
                                                  uint64_t nq, uint32_t ef_search, uint32_t k, uint32_t* d_out_ids, float* d_out_dist,
                                                  uint32_t* d_out_len) {
-    if (!comm) return fail(IDB_ERR_INVALID_ARG, "comm is null");
-    if (nq == 0) return IDB_OK;
-    if (!d_queries || !d_out_ids || k == 0) return fail(IDB_ERR_INVALID_ARG, "bad argument");
+    idb_status st = check_search_args(Family::sharded, shards, n_shards, comm, nullptr, d_queries, nq, d_out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
     ShardLocks locks;
-    idb_status st = locks.lock(shards, n_shards);
-    if (st != IDB_OK) return st;
-    return sharded_search_locked(reinterpret_cast<Index* const*>(shards), n_shards, reinterpret_cast<Comm*>(comm), d_queries, nq, ef_search,
-                                 k, d_out_ids, d_out_dist, d_out_len);
+    if ((st = locks.lock(shards, n_shards)) != IDB_OK) return st;
+    return sharded_search_locked(reinterpret_cast<Index* const*>(shards), n_shards, reinterpret_cast<Comm*>(comm), d_queries, false, nq,
+                                 ef_search, k, d_out_ids, d_out_dist, d_out_len);
 }
 
 idb_status idb_sharded_search_batch_device(idb_index* index, idb_comm* comm, const float* d_queries, uint64_t nq, uint32_t ef_search,
@@ -227,39 +224,22 @@ idb_status idb_sharded_search_batch_device(idb_index* index, idb_comm* comm, con
 
 idb_status idb_sharded_search_batch_f32_multi(idb_index* const* shards, uint32_t n_shards, idb_comm* comm, const float* queries, uint64_t nq,
                                               uint32_t ef_search, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len) {
-    if (!comm) return fail(IDB_ERR_INVALID_ARG, "comm is null");
-    if (nq == 0) return IDB_OK;
-    if (!queries || !out_ids || k == 0) return fail(IDB_ERR_INVALID_ARG, "bad argument");
+    idb_status st = check_search_args(Family::sharded, shards, n_shards, comm, nullptr, queries, nq, out_ids, k);
+    if (st != IDB_OK || nq == 0) return st;
     ShardLocks locks;  // held across staging, search and copy-back: the staging buffers belong to this call
-    idb_status st = locks.lock(shards, n_shards);
-    if (st != IDB_OK) return st;
+    if ((st = locks.lock(shards, n_shards)) != IDB_OK) return st;
     Index* ix = reinterpret_cast<Index*>(shards[0]);
     Lane& ln = ix->lanes[0];
     CUDA_TRY(cudaSetDevice(ix->device));
-    CUDA_TRY(ensure_f32(ln.q2, ln.q2_cap, nq * ix->dim));
-    CUDA_TRY(ensure_u32(ln.ids2, ln.ids2_cap, nq * k));
+    CUDA_TRY(ensure_u32(ln.ids, ln.ids_cap, nq * k));
     CUDA_TRY(ensure_f32(ln.dist, ln.dist_cap, nq * k));
     CUDA_TRY(ensure_u32(ln.len, ln.len_cap, nq));
-    CUDA_TRY(cudaMemcpyAsync(ln.q2, queries, nq * ix->dim * 4, cudaMemcpyHostToDevice, ln.stream));
-    st = sharded_search_locked(reinterpret_cast<Index* const*>(shards), n_shards, reinterpret_cast<Comm*>(comm), ln.q2, nq, ef_search, k,
-                               ln.ids2, ln.dist, ln.len);
+    st = sharded_search_locked(reinterpret_cast<Index* const*>(shards), n_shards, reinterpret_cast<Comm*>(comm), queries, true, nq,
+                               ef_search, k, ln.ids, ln.dist, ln.len);
     if (st != IDB_OK) return st;
-    HostOut ho;  // (pageable output buffers are staged through pinned memory: internal.cuh)
-    ho.add(out_ids, ln.ids2, nq * k * 4);
-    ho.add(out_dist, ln.dist, nq * k * 4);
-    ho.add(out_len, ln.len, nq * 4);
-    CUDA_TRY(ho.enqueue(ln));
-    CUDA_TRY(cudaStreamSynchronize(ln.stream));  // every shard's stream was joined into this one
-    ho.finish();
-    uint32_t failed = 0;
-    for (uint32_t i = 0; i < n_shards; ++i) {
-        Lane& sl = reinterpret_cast<Index*>(shards[i])->lanes[0];
-        SearchCtrl ctrl = {};
-        if (sl.ctrl && sl.last_nq) CUDA_TRY(cudaMemcpy(&ctrl, sl.ctrl, sizeof(ctrl), cudaMemcpyDeviceToHost));
-        failed += ctrl.retry.fail_count;
-    }
-    if (failed) return fail(IDB_ERR_CAPACITY, "%u queries overflowed an internal per-query structure on this rank's shards", failed);
-    return IDB_OK;
+    std::vector<Lane*> lanes;  // every shard's stream was joined into ln's
+    for (Index* sx : locks.order) lanes.push_back(&sx->lanes[0]);
+    return read_back(ln, nq, k, out_ids, out_dist, out_len, lanes.data(), (uint32_t)lanes.size());
 }
 
 idb_status idb_sharded_search_batch_f32(idb_index* index, idb_comm* comm, const float* queries, uint64_t nq, uint32_t ef_search, uint32_t k,
