@@ -714,6 +714,8 @@ GraphView Index::view() const {
     g.flags = opt_flags;
     g.codes = d_codes;
     g.cparams = d_cparams;
+    g.cstep = code_step;
+    g.cerr = code_err;
     return g;
 }
 

@@ -49,6 +49,8 @@ struct GraphView {
     // Screening table (DESIGN §2, §4), or null: K1 then fetches every candidate row in full.
     const uint32_t* codes;       // n rows of nchunks u32: word c holds the 8-bit codes of elements 4c..4c+3 (byte k = element 4c+k)
     const float4* cparams;       // 3 x nchunks float4: per element scale, offset, E (x~ = fmaf(code, scale, offset), |x - x~| <= E)
+    float cstep;                 // S: the one code step of every element (the scale slots of cparams all hold it)
+    float cerr;                  // R >= ||x - x~|| over every stored row, x~_i = offset_i + code_i * S in real arithmetic
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -167,19 +169,21 @@ __device__ __forceinline__ float butterfly_sum(float s) {
 // log2(NB) stages are "transposing" (each lane hands half of its values to its partner and keeps the other half,
 // split by even/odd index), so NB vectors cost NB-1 shuffles instead of 5*NB; the remaining stages are plain.
 // Same add tree as butterfly_sum for every vector.  On return lane l holds the total of vector (l & (NB-1)).
-// kDown: every add rounds toward -inf instead (the screening bound, which must never exceed the exact sum).
+// kDown: every add rounds toward -inf instead.  u32 partials (the screen's squared code distances) add exactly, in any order.
 template <bool kDown>
 __device__ __forceinline__ float fadd_dir(float a, float b) { return kDown ? __fadd_rd(a, b) : __fadd_rn(a, b); }
-template <int NB, bool kDown = false>
-__device__ __forceinline__ float batch_butterfly(float (&p)[NB], int lane) {
+template <bool kDown>
+__device__ __forceinline__ uint32_t fadd_dir(uint32_t a, uint32_t b) { return a + b; }
+template <int NB, bool kDown = false, class T = float>
+__device__ __forceinline__ T batch_butterfly(T (&p)[NB], int lane) {
     int off = 1;
 #pragma unroll
     for (int m = NB; m > 1; m >>= 1) {
         const bool up = (lane & off) != 0;
 #pragma unroll
         for (int i = 0; i < m / 2; ++i) {
-            float send = up ? p[2 * i] : p[2 * i + 1];
-            float keep = up ? p[2 * i + 1] : p[2 * i];
+            T send = up ? p[2 * i] : p[2 * i + 1];
+            T keep = up ? p[2 * i + 1] : p[2 * i];
             p[i] = fadd_dir<kDown>(keep, __shfl_xor_sync(kFullMask, send, off));
         }
         off <<= 1;
@@ -736,54 +740,70 @@ __device__ __forceinline__ void batch_distances(const GraphView& g, const QVec<C
 
 // ---------------------------------------------------------------------------------------------------------
 // Screening (DESIGN §4 "screen"): a lower bound of a candidate's canonical distance from its 8-bit codes (128 B per row at dim 128
-// instead of 512 B), so that rows the admission test would reject anyway are never fetched in full.
-//   x~_i = fmaf(code_i, scale_i, offset_i) (round to nearest), E_i >= |x_i - x~_i| over every stored row;
-//   a_i  = max(0, |q_i - x~_i|_rz - E_i)_rd <= |q_i - x_i|,   LB = sum_rd a_i^2 <= sum (q_i - x_i)^2 (exact);
-//   bound = LB * (1 - 2^-16)_rd if that is > 2^-100, else 0.  bound > dist(furthest)  =>  canonical distance > dist(furthest).
-// The factor covers the canonical order's roundings (at most CH + 9 per term, CH <= 8), the floor its underflow; NaN bounds are 0.
+// instead of 512 B), so that rows the admission test would reject anyway are never fetched in full.  Every element shares one code
+// step S (GraphView::cstep), so the bound is a triangle inequality in code space, in integer SIMD:
+//   x~_i = offset_i + c_i S, q^_i = offset_i + qc_i S (real arithmetic), R >= ||x - x~|| for every stored row (GraphView::cerr),
+//   r_q >= ||q - q^|| (ScreenQuery, once per layer), D = sum (qc_i - c_i)^2 (VABSDIFF4 + IDP.4A, exact in u32), so
+//   ||q - x|| >= ||q^ - x~|| - r_q - R = S sqrt(D) - r_q - R,  bound = ((S sqrt(D))_rd - (r_q + R)_ru)_+^2 rounded down,
+//   then * (1 - 2^-16)_rd and 0 below 2^-100.  bound > dist(furthest)  =>  canonical distance > dist(furthest).
+// The factor covers the canonical order's roundings (at most CH + 9 per term, CH <= 8), the floor its underflow; a NaN or infinite
+// query element makes r_q NaN / inf and the bound 0.
 // ---------------------------------------------------------------------------------------------------------
 constexpr float kScreenKeep = 0.9999847412109375f;  // 1 - 2^-16, exact
 constexpr float kScreenFloor = 0x1p-100f;
-// Code byte k of w as a float, exactly: 0x4B0000cc is 2^23 + c.
-__device__ __forceinline__ float code_of(uint32_t w, int k) {
-    return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7540u | (uint32_t)k)), 8388608.f);
-}
-__device__ __forceinline__ float screen_term(float q, float code, float scale, float offset, float e, float acc) {
-    const float d = fabsf(__fsub_rz(q, __fmaf_rn(code, scale, offset)));  // <= |q - x~|
-    const float a = fmaxf(__fsub_rd(d, e), 0.f);                          // <= |q - x|  (a NaN query element gives 0)
-    return __fmaf_rd(a, a, acc);
-}
-// Scale / offset / E of chunk c (zeros beyond the row: those elements contribute 0).  Loaded per use, from L1: keeping them in
-// registers for all CH chunks would not fit next to the query.
-struct ScreenChunk {
-    float4 sc, of, er;
-};
-__device__ __forceinline__ ScreenChunk screen_chunk_params(const GraphView& g, uint32_t c, bool ok) {
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    ScreenChunk p;
-    p.sc = ok ? __ldg(g.cparams + c) : z;
-    p.of = ok ? __ldg(g.cparams + g.nchunks + c) : z;
-    p.er = ok ? __ldg(g.cparams + 2 * g.nchunks + c) : z;
-    return p;
-}
-// acc + this lane's four terms of one chunk (query chunk q, code word w).
-__device__ __forceinline__ float screen_chunk(const float4& q, uint32_t w, const ScreenChunk& p, float acc) {
-    acc = screen_term(q.x, code_of(w, 0), p.sc.x, p.of.x, p.er.x, acc);
-    acc = screen_term(q.y, code_of(w, 1), p.sc.y, p.of.y, p.er.y, acc);
-    acc = screen_term(q.z, code_of(w, 2), p.sc.z, p.of.z, p.er.z, acc);
-    return screen_term(q.w, code_of(w, 3), p.sc.w, p.of.w, p.er.w, acc);
-}
 __device__ __forceinline__ float screen_finish(float lb) {
     const float b = __fmul_rd(lb, kScreenKeep);
     return b > kScreenFloor ? b : 0.f;
+}
+// The query side of the bound: this lane's codes qc (word j = elements 4c..4c+3 of chunk c = lane + 32 j, packed as the table's
+// words) and slack = (r_q + R) rounded up.  Computed once per layer; the retry pass re-runs the layers, so it recomputes it.
+template <int CH>
+struct ScreenQuery {
+    uint32_t qc[CH];
+    float slack;
+};
+template <int CH>
+__device__ __forceinline__ void screen_query(ScreenQuery<CH>& sq, const GraphView& g, const float4 (&q)[CH], int lane) {
+    const float S = g.cstep;
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < CH; ++j) {
+        const uint32_t c = lane + 32 * j;
+        const float4 of = c < g.nchunks ? __ldg(g.cparams + g.nchunks + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        const float qv[4] = {q[j].x, q[j].y, q[j].z, q[j].w}, ov[4] = {of.x, of.y, of.z, of.w};
+        uint32_t w = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            // any code in [0, 255] is valid (r_q measures the one chosen); a NaN element gets 0
+            const float code = S > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(qv[k], ov[k]), S)), 0.f), 255.f) : 0.f;
+            // q^ lies in [fmaf_rd, fmaf_ru]: |q - q^| <= max(q - lo, hi - q), both rounded up (NaN / inf propagate)
+            const float d = fmaxf(__fsub_ru(qv[k], __fmaf_rd(code, S, ov[k])), __fsub_ru(__fmaf_ru(code, S, ov[k]), qv[k]));
+            acc = __fmaf_ru(d, d, acc);
+            w |= (uint32_t)code << (8 * k);
+        }
+        sq.qc[j] = w;
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) acc = __fadd_ru(acc, __shfl_xor_sync(kFullMask, acc, o));
+    sq.slack = __fadd_ru(__fsqrt_ru(acc), g.cerr);
+}
+// The bound from a row's squared code distance D (all lanes of the warp agree on slack).
+__device__ __forceinline__ float screen_bound_of(const GraphView& g, uint32_t D, float slack) {
+    const float t = fmaxf(__fsub_rd(__fmul_rd(g.cstep, __fsqrt_rd(__uint2float_rd(D))), slack), 0.f);  // NaN slack: 0
+    return screen_finish(__fmul_rd(t, t));
+}
+// acc + sum over this lane's four elements of (qc - c)^2: one VABSDIFF4 and one IDP.4A per code word.
+__device__ __forceinline__ uint32_t screen_word(uint32_t qc, uint32_t w, uint32_t acc) {
+    const uint32_t d = __vabsdiffu4(w, qc);
+    return __dp4a(d, d, acc);
 }
 template <int CH>
 __device__ __forceinline__ constexpr int screen_rows() { return CH == 1 ? 32 : CH == 2 ? 16 : CH <= 4 ? 8 : 2; }  // code words in flight <= 32
 // Drops the candidates in cpid[0, n_new) whose bound exceeds fdist (the distance of the ef-th key of nearest) and compacts the rest,
 // in row order, to the front of cpid.  Returns how many are left.  Warp-uniform call.
 template <int CH, bool kFull>
-__device__ __forceinline__ uint32_t screen_candidates(WarpState& s, const GraphView& g, const float4 (&q)[CH], uint32_t n_new, float fdist,
-                                                      int lane) {
+__device__ __forceinline__ uint32_t screen_candidates(WarpState& s, const GraphView& g, const ScreenQuery<CH>& sq, uint32_t n_new,
+                                                      float fdist, int lane) {
     uint32_t* cpid = s.cpid;
     constexpr int NS = screen_rows<CH>();
     bool cok[CH];
@@ -820,16 +840,14 @@ __device__ __forceinline__ uint32_t screen_candidates(WarpState& s, const GraphV
         }
 #endif
         const uint32_t mine = (uint32_t)lane < (uint32_t)NS && (uint32_t)lane < nb ? cpid[b0 + lane] : kInvalid;
-        float p[NS];
+        uint32_t p[NS];
 #pragma unroll
-        for (int i = 0; i < NS; ++i) p[i] = 0.f;
+        for (int i = 0; i < NS; ++i) p[i] = 0u;
 #pragma unroll
-        for (int j = 0; j < CH; ++j) {
-            const ScreenChunk pc = screen_chunk_params(g, lane + 32 * j, cok[j]);
+        for (int j = 0; j < CH; ++j)
 #pragma unroll
-            for (int i = 0; i < NS; ++i) p[i] = screen_chunk(q[j], w[i][j], pc, p[i]);
-        }
-        const float bound = screen_finish(batch_butterfly<NS, true>(p, lane));  // lane l: row b0 + (l & (NS - 1))
+            for (int i = 0; i < NS; ++i) p[i] = screen_word(sq.qc[j], w[i][j], p[i]);
+        const float bound = screen_bound_of(g, batch_butterfly<NS>(p, lane), sq.slack);  // lane l: row b0 + (l & (NS - 1))
         const bool keep = mine != kInvalid && !(bound > fdist);
         const uint32_t m = __ballot_sync(kFullMask, keep);
         __syncwarp();  // every lane has read this batch's ids before any is overwritten (writes go to [kept, b0 + NS))
@@ -983,6 +1001,11 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
 #ifdef IDB_K1_PHASES
     k1_phase_begin(s);
 #endif
+    constexpr bool kScreen = SCREEN && CH > 0 && !kLive && !TMA;
+    ScreenQuery<kScreen ? CH : 1> sq;
+    if constexpr (kScreen) {
+        if (g.codes) screen_query<CH>(sq, g, q.r, lane);
+    }
     for (;;) {
         uint64_t* near = (s.near_base + s.cur * s.near_len);
         uint32_t n_new = 0;
@@ -1091,9 +1114,9 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
             __syncwarp();
             // ---- screen (DESIGN §4): with nearest full, a candidate whose code bound exceeds the furthest distance has a key
             // above the furthest key, so it would not be admitted; only the others are fetched in full, still in row order --------
-            if constexpr (SCREEN && CH > 0 && !kLive && !TMA) {
+            if constexpr (kScreen) {
                 if (g.codes && s.cnt >= ef_cur) {
-                    n_new = screen_candidates<CH, FULL>(s, g, q.r, n_new, __uint_as_float(key_dbits(near[s.cnt - 1])), lane);
+                    n_new = screen_candidates<CH, FULL>(s, g, sq, n_new, __uint_as_float(key_dbits(near[s.cnt - 1])), lane);
                     if (n_new == 0) continue;
                 }
             }

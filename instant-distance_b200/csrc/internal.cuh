@@ -216,10 +216,13 @@ struct Index {
     const uint32_t** d_upper_ptrs = nullptr;   // device copy of the pointer table
     uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map)
     bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
-    // Screening table of the stored rows (DESIGN §2, §4): n x nchunks u32 of 8-bit codes + 3 x nchunks float4 (scale, offset, E).
+    // Screening table of the stored rows (DESIGN §2, §4): n x nchunks u32 of 8-bit codes + 3 x nchunks float4 (scale, offset, E),
+    // one code step for every element and the bound on every row's coding error (GraphView::cstep / cerr).
     // Null when screening is off (IDB_SCREEN=0), the index is empty, or a stored value is not finite.
     uint32_t* d_codes = nullptr;
     float4* d_cparams = nullptr;
+    float code_step = 0.f;
+    float code_err = 0.f;
     bool screen = true;                        // IDB_SCREEN (default 1): build the table and let K1 screen with it; never changes results
 
     // tuning knobs (env IDB_OPT / IDB_VIS_MULT / IDB_VIS_TIER / IDB_B16_BYTES / IDB_VIS_SLOTS / IDB_VARIANT); none of them changes results

@@ -1,12 +1,16 @@
 // screen.cu — the per-index screening table K1 uses to skip candidate rows it would reject (DESIGN §2, §4), and a diagnostic entry
 // point that evaluates the screening bound next to the canonical distance for given (query, row) pairs.
 //
-// Table: per element i of a row (dim rounded up to 4, as the stored rows), an affine 8-bit code  x~ = fmaf(code, scale_i, offset_i)
-// (round to nearest) with scale_i = max_i / 255 - min_i / 255 and offset_i = min_i over the stored rows, and E_i = max over the rows
-// of |x - x~| rounded up, measured on the device with the same fmaf the screen uses — so |x - x~| <= E_i holds for every stored
-// value by construction, whatever the rounding of the codes.
+// Table: one code step S for every element and a per-element offset_i = min_i over the stored rows, codes
+// c_i = clamp(rint((x_i - offset_i) / S), 0, 255) with S >= max_i (max_i - min_i) / 255 (rounded up), so that code differences
+// measure distance in the same unit everywhere: ||q^ - x~|| = S * sqrt(sum (qc_i - c_i)^2) exactly, where x~_i = offset_i + c_i * S
+// in real arithmetic (K1's integer bound, hnsw_device.cuh screen_candidates).  Beside the codes:
+//   R   >= ||x - x~|| over every stored row, measured on the device with upward rounding (x~ bracketed by fmaf_rd / fmaf_ru);
+//   E_i  = max over the rows of |x - fmaf_rn(c, S, offset_i)| rounded up, and S in every scale slot, so the per-element float bound
+//          |q_i - x~_i| - E_i <= |q_i - x_i| holds on the same codes.
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <vector>
 
 #include "internal.cuh"
@@ -45,37 +49,74 @@ __global__ void code_range_kernel(const void* pts, uint32_t bf16, uint64_t n, ui
     }
 }
 
-// prm: [0, stride) scale, [stride, 2 stride) offset; [2 stride, 3 stride) E is zeroed here and filled by code_encode_kernel.
-__global__ void code_params_kernel(const uint32_t* mn, const uint32_t* mx, uint32_t stride, float* prm) {
+// prm: [0, stride) scale (filled with S by code_encode_kernel), [stride, 2 stride) offset; [2 stride, 3 stride) E is zeroed here and
+// filled by code_encode_kernel.  step: S, the largest per-element step (hi - lo) / 255 rounded up (atomicMax of non-negative floats).
+__global__ void code_params_kernel(const uint32_t* mn, const uint32_t* mx, uint32_t stride, float* prm, uint32_t* step) {
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= stride) return;
     const float lo = float_of_ord(mn[e]), hi = float_of_ord(mx[e]);
-    float scale = __fsub_rn(__fdiv_rn(hi, 255.f), __fdiv_rn(lo, 255.f));  // (hi - lo) / 255 without overflow for finite hi, lo
-    if (!(scale > 0.f)) scale = 0.f;                                       // a constant element: every code decodes to offset
-    prm[e] = scale;
+    float scale = __fsub_ru(__fdiv_ru(hi, 255.f), __fdiv_rd(lo, 255.f));  // >= (hi - lo) / 255 without overflow for finite hi, lo
+    if (!(scale > 0.f)) scale = 0.f;                                       // a constant element
+    atomicMax(step, __float_as_uint(scale));
     prm[stride + e] = lo;
     prm[2 * stride + e] = 0.f;
 }
 
+__device__ __forceinline__ float code_of_value(float x, float offset, float step) {
+    return step > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(x, offset), step)), 0.f), 255.f) : 0.f;
+}
+
 __global__ void code_encode_kernel(const void* pts, uint32_t bf16, uint64_t n, uint32_t stride, uint64_t rows_per_block, float* prm,
-                                   unsigned char* codes) {
+                                   const uint32_t* step, unsigned char* codes) {
+    const float S = __uint_as_float(*step);
+    if (blockIdx.x == 0)
+        for (uint32_t e = threadIdx.x; e < stride; e += blockDim.x) prm[e] = S;
     const uint64_t r0 = (uint64_t)blockIdx.x * rows_per_block, r1 = min(n, r0 + rows_per_block);
     if (r0 >= r1) return;
     for (uint32_t e = threadIdx.x; e < stride; e += blockDim.x) {
-        const float scale = prm[e], offset = prm[stride + e];
+        const float offset = prm[stride + e];
         float err = 0.f;
         for (uint64_t r = r0; r < r1; ++r) {
             const float x = stored_at(pts, bf16, r * stride + e);
-            const float c = scale > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(x, offset), scale)), 0.f), 255.f) : 0.f;
+            const float c = code_of_value(x, offset, S);
             codes[r * stride + e] = (unsigned char)c;
-            const float xt = __fmaf_rn(c, scale, offset);  // the screen's x~ (hnsw_device.cuh screen_term)
+            const float xt = __fmaf_rn(c, S, offset);  // x~ of the per-element float bound
             err = fmaxf(err, __fsub_ru(fmaxf(x, xt), fminf(x, xt)));
         }
         atomicMax(reinterpret_cast<uint32_t*>(prm + 2 * stride + e), __float_as_uint(err));  // non-negative: same order as the floats
     }
 }
 
+// One warp per row (grid-stride): r_x = ||x - x~||, rounded up, with x~_i = offset_i + c_i * S in real arithmetic, which lies in
+// [fmaf_rd(c, S, offset), fmaf_ru(c, S, offset)], so |x_i - x~_i| <= max(x_i - lo, hi - x_i).  err_max = max over the rows.
+__global__ void code_row_err_kernel(const void* pts, uint32_t bf16, uint64_t n, uint32_t nchunks, const float* prm,
+                                    const uint32_t* step, const uint32_t* codes, uint32_t* err_max) {
+    const float S = __uint_as_float(*step);
+    const uint32_t stride = nchunks * 4;
+    const int lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
+    float worst = 0.f;
+    for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < n; r += warps) {
+        float acc = 0.f;
+        for (uint32_t c = lane; c < nchunks; c += 32) {
+            const uint32_t w = codes[r * nchunks + c];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint32_t e = 4 * c + k;
+                const float x = stored_at(pts, bf16, r * stride + e), off = prm[stride + e], code = (float)((w >> (8 * k)) & 0xFFu);
+                const float d = fmaxf(__fsub_ru(x, __fmaf_rd(code, S, off)), __fsub_ru(__fmaf_ru(code, S, off), x));
+                acc = __fmaf_ru(d, d, acc);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) acc = __fadd_ru(acc, __shfl_xor_sync(kFullMask, acc, o));
+        worst = fmaxf(worst, __fsqrt_ru(acc));
+    }
+    if (lane == 0) atomicMax(err_max, __float_as_uint(worst));
+}
+
 // One warp per (query, row) pair: the screen's bound (what K1 compares with the furthest distance) and the canonical distance.
+// The same helpers as K1's screen_candidates: screen_query, screen_word, batch_butterfly, screen_bound_of.
 template <int CH, class RT>
 __global__ void screen_bound_kernel(GraphView g, const float4* queries, const uint32_t* pairs, uint64_t npairs, float* out_bound,
                                     float* out_dist) {
@@ -88,14 +129,15 @@ __global__ void screen_bound_kernel(GraphView g, const float4* queries, const ui
     float4 x[CH];
     load_row<CH, RT>(g, pid, lane, x);
     const float dist = butterfly_sum(lane_partial<CH>(q.r, x));
-    float p[1] = {0.f};
+    ScreenQuery<CH> sq;
+    screen_query<CH>(sq, g, q.r, lane);
+    uint32_t p[1] = {0u};
 #pragma unroll
     for (int j = 0; j < CH; ++j) {
         const uint32_t c = lane + 32 * j;
-        const uint32_t cw = c < g.nchunks ? g.codes[(size_t)pid * g.nchunks + c] : 0u;
-        p[0] = screen_chunk(q.r[j], cw, screen_chunk_params(g, c, c < g.nchunks), p[0]);
+        p[0] = screen_word(sq.qc[j], c < g.nchunks ? g.codes[(size_t)pid * g.nchunks + c] : 0u, p[0]);
     }
-    const float bound = screen_finish(batch_butterfly<1, true>(p, lane));
+    const float bound = screen_bound_of(g, batch_butterfly<1>(p, lane), sq.slack);
     if (lane == 0) {
         out_bound[w] = bound;
         out_dist[w] = dist;
@@ -123,12 +165,12 @@ idb_status Index::build_codes() {
     const void* pts = bf16 ? static_cast<const void*>(d_points_bf16) : static_cast<const void*>(d_points);
     const unsigned grid = (unsigned)std::min<uint64_t>((n + 63) / 64, (uint64_t)num_sms * 8);
     const uint64_t rows_per_block = (n + grid - 1) / grid;
-    uint32_t* tmp = nullptr;  // [0, stride) min, [stride, 2 stride) max, [2 stride] non-finite flag
-    CUDA_TRY(cudaMalloc(&tmp, (2 * (size_t)stride + 1) * 4));
+    uint32_t* tmp = nullptr;  // [0, stride) min, [stride, 2 stride) max, [2 stride] non-finite flag, [2 stride + 1] S, [2 stride + 2] R
+    CUDA_TRY(cudaMalloc(&tmp, (2 * (size_t)stride + 3) * 4));
     cudaError_t e = cudaMalloc(&d_cparams, 3 * (size_t)stride * 4);
     if (e == cudaSuccess) e = cudaMalloc(&d_codes, n * (size_t)stride);
     if (e == cudaSuccess) e = fill_u32(tmp, stride, 0xFFFFFFFFu, stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(tmp + stride, 0, ((size_t)stride + 1) * 4, stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(tmp + stride, 0, ((size_t)stride + 3) * 4, stream);
     if (e == cudaSuccess) {
         code_range_kernel<<<grid, 128, 0, stream>>>(pts, bf16 ? 1u : 0u, n, stride, rows_per_block, tmp, tmp + stride, tmp + 2 * stride);
         e = cudaGetLastError();
@@ -136,14 +178,20 @@ idb_status Index::build_codes() {
     uint32_t bad = 0;
     if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, tmp + 2 * stride, 4, cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    uint32_t step_err[2] = {0u, 0u};
     if (e == cudaSuccess && !bad) {
         float* prm = reinterpret_cast<float*>(d_cparams);
-        code_params_kernel<<<(stride + 127) / 128, 128, 0, stream>>>(tmp, tmp + stride, stride, prm);
-        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, bf16 ? 1u : 0u, n, stride, rows_per_block, prm,
+        uint32_t* step = tmp + 2 * stride + 1;
+        code_params_kernel<<<(stride + 127) / 128, 128, 0, stream>>>(tmp, tmp + stride, stride, prm, step);
+        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, bf16 ? 1u : 0u, n, stride, rows_per_block, prm, step,
                                                      reinterpret_cast<unsigned char*>(d_codes));
+        code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(pts, bf16 ? 1u : 0u, n, nchunks, prm, step, d_codes, step + 1);
         e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaMemcpyAsync(step_err, step, 8, cudaMemcpyDeviceToHost, stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     }
+    std::memcpy(&code_step, &step_err[0], 4);
+    std::memcpy(&code_err, &step_err[1], 4);
     cudaFree(tmp);
     if (e != cudaSuccess || bad) {  // a non-finite stored value: no table, K1 fetches every row in full
         cudaFree(d_codes);
