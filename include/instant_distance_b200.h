@@ -94,6 +94,33 @@ IDB_API idb_status idb_build_f32(const float* rows, uint64_t n, uint32_t dim, co
 IDB_API idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, const idb_params* params, uint32_t metric,
                                 idb_index** out_index, uint32_t* out_ids);
 
+/* Insert: append m host rows (m x dim f32) to an index of n0 points, each by Construction::insert(new, 0, layers) (core:437-528):
+ * a descent from the top layer with ef = 1 on the layer snapshots, ef_construction on layer 0, select_heuristic (or the simple
+ * selection), then the re-pruning of every target row.
+ *   - PointIds: the new points get n0 .. n0+m-1 in input order (no shuffle); out_ids[i] = n0 + i (may be NULL).
+ *   - Layer 0 only.  Layer l holds exactly PointIds [0, n_l) (core:275-281), so a new point could enter an upper layer only by
+ *     renumbering existing ones, which this call does not do.  The upper layers, their snapshots and ef_search do not change: they
+ *     stay a sample of the first n0 points, so navigation can degrade as m / n0 grows (DESIGN.md §6a: no recall loss measured up to
+ *     m = n0 on sift-shaped rows).
+ *   - Batches: the build's layer-0 schedule from g0 = n0, b = min(max_batch, max(1, g0 / growth)) with max_batch / growth from
+ *     insert_batch (1 = the sequential reference order), else IDB_BUILD_MAXBATCH / IDB_BUILD_GROWTH (defaults 16384 / 8).  Unlike
+ *     the build, an index with no upper layer is also inserted into in batches.  An empty index (n0 = 0) makes the first row its
+ *     entry point, PointId 0.
+ *   - Rows are stored as the build stores them: zero padded, normalised for a cosine index, then narrowed for a bf16 one.
+ *   - params: ef_construction (1..1024), heuristic, keep_pruned, insert_batch and progress (called with the rows inserted so far
+ *     and m) are read; M must equal the index's M; extend_candidates is refused as by the build; seed, ml, ef_search, storage and
+ *     device are ignored.  dim must equal the index's dim; n0 + m >= u32::MAX is refused (core:256); m = 0 does nothing.
+ *   - global_ids (m entries): required when the index has an id map (idb_index_set_id_map), refused when it has none; appended to
+ *     the map, so a shard keeps reporting global ids.
+ *   - Exclusive (&mut self): searches on other threads wait until the insert has finished and see the index before or after it.
+ *   - Failures: an argument error, a failed allocation or a CUDA error before the first batch leaves the index as it was.
+ *     IDB_ERR_CAPACITY (an insert overflowed even the retry pass, e.g. in a cluster of thousands of identical rows): the index keeps
+ *     the batches before the failing one — n is then that batch's first PointId — and stays searchable.  The traversals see
+ *     n = n0 + m for the whole call.
+ *   - Storage doubles when it grows, so repeated small inserts are not quadratic.  The screening table is rebuilt from all rows. */
+IDB_API idb_status idb_index_insert_f32(idb_index* index, const float* rows, uint64_t m, uint32_t dim, const idb_params* params,
+                                        const uint32_t* global_ids, uint32_t* out_ids);
+
 /* "Search a given graph": adopt a graph built elsewhere (the reference, the oracle, a loaded .idx file).
  * This is the parity entry point.  Mirrors the fields of `Hnsw` (core:194-199):
  *   points   n x dim, PointId order                       (Hnsw::points)

@@ -127,6 +127,41 @@ class Hnsw {
         if (i >= s.len_) return std::nullopt;
         return Item{s.dist_[i], PointId{s.ids_[i]}, &points_[s.ids_[i]]};
     }
+    // Not in the reference: Construction::insert (core:437-528) of each point on layer 0 (idb_index_insert_f32); returns their
+    // PointIds, which continue from the current count in input order.  Like a `&mut self` method it invalidates the Items of
+    // earlier searches (their points move when points_ grows).  On IDB_ERR_CAPACITY the index keeps the batches before the failing
+    // one; their points are appended to points_ before the Error is thrown, so points_ always has one entry per PointId.
+    std::vector<PointId> insert(std::vector<Point> points, size_t ef_construction = 100,
+                                std::optional<Heuristic> heuristic = Heuristic{}) {
+        idb_info info;
+        check(idb_index_info(raw_, &info));
+        std::vector<float> flat;
+        flat.reserve(points.size() * info.dim);
+        for (const Point& p : points) {
+            if (p.v.size() != info.dim) throw Error(IDB_ERR_INVALID_ARG, "point dimension differs from the index");
+            flat.insert(flat.end(), p.v.begin(), p.v.end());
+        }
+        idb_params p;
+        check(idb_params_default(&p));
+        p.M = info.M;
+        p.ef_construction = (uint32_t)ef_construction;
+        p.heuristic = heuristic ? 1 : 0;
+        p.extend_candidates = heuristic && heuristic->extend_candidates;
+        p.keep_pruned = !heuristic || heuristic->keep_pruned;
+        std::vector<uint32_t> ids(points.size());
+        const idb_status st = idb_index_insert_f32(raw_, flat.data(), points.size(), info.dim, &p, nullptr, ids.data());
+        if (st != IDB_OK) {
+            const Error err(st, idb_last_error());
+            idb_info now;
+            if (idb_index_info(raw_, &now) == IDB_OK)
+                for (uint64_t i = 0; i < now.n - info.n && i < points.size(); ++i) points_.push_back(std::move(points[i]));
+            throw err;
+        }
+        std::vector<PointId> out(points.size());
+        for (size_t i = 0; i < points.size(); ++i) out[i] = PointId{ids[i]};
+        for (Point& pt : points) points_.push_back(std::move(pt));
+        return out;
+    }
     // lib.rs:386-391, types.rs:269-275
     const std::vector<Point>& iter() const { return points_; }
     const Point& operator[](PointId p) const { return points_.at(p.raw); }
@@ -148,6 +183,20 @@ class HnswMap {
         return out;
     }
     const std::vector<Point>& iter() const { return hnsw_.iter(); }
+    // Hnsw::insert, with one value per point, appended in PointId order.
+    std::vector<PointId> insert(std::vector<Point> points, std::vector<V> vals, size_t ef_construction = 100,
+                                std::optional<Heuristic> heuristic = Heuristic{}) {
+        if (vals.size() != points.size()) throw Error(IDB_ERR_INVALID_ARG, "points and values differ in length");
+        const size_t n0 = hnsw_.iter().size();
+        try {
+            std::vector<PointId> ids = hnsw_.insert(std::move(points), ef_construction, heuristic);
+            for (V& v : vals) values.push_back(std::move(v));
+            return ids;
+        } catch (const Error&) {  // values follow PointIds, also for the points a failed insert kept
+            for (size_t i = 0; i < hnsw_.iter().size() - n0; ++i) values.push_back(std::move(vals[i]));
+            throw;
+        }
+    }
 };
 
 // lib.rs:21-113

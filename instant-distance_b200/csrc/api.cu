@@ -673,13 +673,69 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, 
 idb_status Index::narrow_points_to_bf16() {
     const size_t total = n * (size_t)nchunks * 4;
     if (total == 0) { bf16 = true; return IDB_OK; }
-    CUDA_TRY(cudaMalloc(&d_points_bf16, total * 2));
+    CUDA_TRY(cudaMalloc(&d_points_bf16, cap * (size_t)nchunks * 4 * 2));
     narrow_bf16_kernel<<<num_sms * 8, 256, 0, stream>>>(d_points, d_points_bf16, total);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(stream));
     cudaFree(d_points);
     d_points = nullptr;
     bf16 = true;
+    return IDB_OK;
+}
+
+idb_status Index::reserve_rows(uint64_t rows) {
+    if (rows <= cap) return IDB_OK;
+    const uint64_t want = std::max<uint64_t>(rows, 2 * cap);
+    const size_t stride = (size_t)nchunks * 4, width = 2 * (size_t)M;
+    void* pts = nullptr;
+    uint32_t* zero = nullptr;
+    uint32_t* id_map = nullptr;
+    cudaError_t e = cudaMalloc(&pts, want * stride * (bf16 ? 2 : 4));
+    if (e == cudaSuccess) e = cudaMalloc(&zero, want * width * 4);
+    if (e == cudaSuccess && d_id_map) e = cudaMalloc(&id_map, want * 4);
+    if (e == cudaSuccess && n) {
+        e = cudaMemcpyAsync(pts, bf16 ? static_cast<const void*>(d_points_bf16) : static_cast<const void*>(d_points),
+                            n * stride * (bf16 ? 2 : 4), cudaMemcpyDeviceToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(zero, d_zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
+        if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(id_map, d_id_map, n * 4, cudaMemcpyDeviceToDevice, stream);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) {
+        cudaFree(pts);
+        cudaFree(zero);
+        cudaFree(id_map);
+        CUDA_TRY(e);
+    }
+    cudaFree(d_points);
+    cudaFree(d_points_bf16);
+    cudaFree(d_zero);
+    cudaFree(d_id_map);
+    d_points = bf16 ? nullptr : static_cast<float*>(pts);
+    d_points_bf16 = bf16 ? static_cast<uint16_t*>(pts) : nullptr;
+    d_zero = zero;
+    d_id_map = id_map;
+    cap = want;
+    return IDB_OK;
+}
+
+idb_status Index::stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids) {
+    const size_t stride = (size_t)nchunks * 4;
+    float* tmp = nullptr;  // the rows in the kernel layout, f32
+    CUDA_TRY(cudaMalloc(&tmp, m * stride * 4));
+    cudaError_t e = cudaMemsetAsync(tmp, 0, m * stride * 4, stream);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(tmp, stride * 4, rows, dim * 4, dim * 4, m, cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess && metric == kMetricCosine) e = normalize_rows(tmp, stride, tmp, m, dim, nchunks, num_sms, stream);
+    if (e == cudaSuccess && bf16) {  // normalised first, then rounded, as the build does
+        narrow_bf16_kernel<<<num_sms * 8, 256, 0, stream>>>(tmp, d_points_bf16 + r0 * stride, m * stride);
+        e = cudaGetLastError();
+    } else if (e == cudaSuccess) {
+        e = cudaMemcpyAsync(d_points + r0 * stride, tmp, m * stride * 4, cudaMemcpyDeviceToDevice, stream);
+    }
+    if (e == cudaSuccess) e = fill_u32(d_zero + r0 * 2 * M, m * 2 * M, kInvalid, stream);
+    if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(d_id_map + r0, global_ids, m * 4, cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    cudaFree(tmp);
+    CUDA_TRY(e);
     return IDB_OK;
 }
 
@@ -755,6 +811,7 @@ idb_status Index::init_device(int dev) {
     if (const char* e = std::getenv("IDB_VIS_MULT")) vis_mult = std::max(1, std::atoi(e));
     if (const char* e = std::getenv("IDB_VARIANT")) variant = std::atoi(e);
     if (const char* e = std::getenv("IDB_VIS_TIER")) vis_tier = std::atoi(e);
+    if (const char* e = std::getenv("IDB_RETRY_SLOTS")) retry_slots_override = std::min(kRetrySlots, next_pow2((uint64_t)std::max(64, std::atoi(e))));
     if (const char* e = std::getenv("IDB_B16_CAP")) b16_cap_16ths = (uint32_t)std::min(14, std::max(1, std::atoi(e)));
     if (const char* e = std::getenv("IDB_B16_BYTES")) b16_bytes_override = (uint32_t)std::max(64, std::atoi(e));
     if (const char* e = std::getenv("IDB_VIS_SLOTS")) vis_slots_override = next_pow2((uint64_t)std::max(64, std::atoi(e)));
@@ -775,6 +832,7 @@ idb_status Index::upload(const float* points, uint64_t n_, uint32_t dim_, uint32
                         (unsigned long long)upper_n_[l], (unsigned long long)below);
     }
     n = n_;
+    cap = n_;
     dim = dim_;
     M = M_;
     ef_search = ef;
@@ -1015,14 +1073,15 @@ idb_status idb_index_info(const idb_index* index, idb_info* out) {
     if (!index || !out) return fail(IDB_ERR_INVALID_ARG, "null argument");
     const Index* ix = reinterpret_cast<const Index*>(index);
     std::memset(out, 0, sizeof(*out));
-    out->n = ix->n;
+    const uint64_t n = ix->n;  // one read: an insert on another thread may change it
+    out->n = n;
     out->dim = ix->dim;
     out->M = ix->M;
     out->ef_search = ix->ef_search;
     out->device = ix->device;
     out->storage = ix->bf16 ? IDB_STORAGE_BF16 : IDB_STORAGE_F32;
-    out->n_layers = ix->n == 0 ? 0 : (uint32_t)ix->d_upper.size() + 1;
-    if (ix->n) out->layer_n[0] = ix->n;
+    out->n_layers = n == 0 ? 0 : (uint32_t)ix->d_upper.size() + 1;
+    if (n) out->layer_n[0] = n;
     for (size_t l = 0; l < ix->upper_n.size() && l + 1 < 32; ++l) out->layer_n[l + 1] = ix->upper_n[l];
     return IDB_OK;
 }

@@ -160,6 +160,156 @@ struct BuildScratch {
     }
 };
 
+// The batch schedule's cap and divisor: a batch at g0 inserts min(max_batch, max(1, g0 / growth)) points.
+void batch_schedule(const idb_params& p, uint32_t* max_batch, uint32_t* growth) {
+    // Defaults: batch <= 16384 and <= 1/8 of the graph keeps recall@10 of the built graph close to the reference algorithm's own
+    // graph (tests/test_gpu_build.py checks it) while giving each batch enough inserts to fill the device.
+    *max_batch = p.insert_batch ? p.insert_batch : 16384u;
+    *growth = 8;  // a batch never exceeds 1/8 of the graph it is inserted into
+    if (!p.insert_batch) {  // tuning knobs for experiments (results stay valid HNSW graphs; determinism per setting)
+        if (const char* e = std::getenv("IDB_BUILD_MAXBATCH")) *max_batch = (uint32_t)std::max(1, std::atoi(e));
+        if (const char* e = std::getenv("IDB_BUILD_GROWTH")) *growth = (uint32_t)std::max(1, std::atoi(e));
+    }
+}
+
+// One batch of concurrent inserts — KA (+ its retry pass) -> K2 -> sort -> segment heads -> K2' — and the scratch it runs in.
+// The build and the insert (idb_index_insert_f32) both drive their batches through run().
+struct BatchRunner {
+    Index* ix = nullptr;
+    BuildScratch bs;
+    BuildArgs a;
+    bool heuristic = true;
+    bool stage = false;
+    uint32_t k2_smem = 0;
+    int k2_ctas_per_sm = 1;
+    // ka_first: read KA's control block back before K2 and stop there when an insert overflowed even the retry pass, so a failing
+    // batch changes no row (the insert's failure semantics).  Otherwise the block is read once, after K2' (the build's flow).
+    bool ka_first = false;
+
+    // Scratch for batches of up to max_b inserts into ix as it stands (ix->view(): rows, n, layers).
+    idb_status init(Index* index, const idb_params& p, uint64_t max_b, bool ka_first_) {
+        ix = index;
+        ka_first = ka_first_;
+        heuristic = p.heuristic != 0;
+        const uint32_t M = ix->M, cap = 2 * M, efc = p.ef_construction;
+        cudaStream_t st = ix->stream;
+        const uint32_t cand_cap = std::max<uint32_t>((efc + 31) / 32 * 32, cap + kNewCap);
+        CUDA_TRY(cudaMalloc(&bs.cand_keys, (size_t)max_b * cand_cap * 8));
+        CUDA_TRY(cudaMalloc(&bs.cand_cnt, (size_t)max_b * 4));
+        CUDA_TRY(cudaMalloc(&bs.pairs, (size_t)max_b * cap * 8));
+        CUDA_TRY(cudaMalloc(&bs.sorted, (size_t)max_b * cap * 8));
+        CUDA_TRY(cudaMalloc(&bs.seg_start, (size_t)max_b * cap * 4));
+        CUDA_TRY(cudaMalloc(&bs.status, (size_t)max_b * 4));
+        CUDA_TRY(cudaMalloc(&bs.fail_list, (size_t)max_b * 4));
+        CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&bs.h_ctrl), sizeof(BuildCtrl), cudaHostAllocDefault));
+        CUDA_TRY(cudaMalloc(&bs.ctrl, sizeof(BuildCtrl)));
+        CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, bs.cub_bytes, bs.pairs, bs.sorted, (int)(max_b * cap), 0, 64, st));
+        CUDA_TRY(cudaMalloc(&bs.cub_tmp, std::max<size_t>(bs.cub_bytes, 16)));
+
+        // Staging the kept rows in shared memory (72 KB per 2-warp CTA -> 6 warps per SM) trades 32 resident warps for 6 to save
+        // reads that L1/L2 serve anyway, so it is off unless asked for.
+        if (const char* e = std::getenv("IDB_BUILD_STAGE")) stage = std::atoi(e) != 0 && SelectSmem::bytes(cand_cap, M, ix->nchunks, true) <= 56 * 1024;
+        k2_smem = (uint32_t)SelectSmem::bytes(cand_cap, M, ix->nchunks, stage);
+        // K2 / K2' are persistent grids of 2-warp CTAs.  They are issue-bound (pairwise distances on L1/L2-resident rows), so the
+        // grid asks for as many CTAs per SM as shared memory (228 KB per SM on an H100) and registers allow, up to 16 (32 warps per SM).
+        k2_ctas_per_sm = (int)std::min<uint64_t>(16, std::max<uint64_t>(1, (200 * 1024) / std::max<uint32_t>(1, k2_smem * kBuildWarps)));
+        if (const char* e = std::getenv("IDB_BUILD_CTAS")) k2_ctas_per_sm = std::max(1, std::atoi(e));
+
+        std::memset(&a, 0, sizeof(a));
+        a.g = ix->view();
+        a.zero = ix->d_zero;
+        a.efc = efc;
+        a.cand_cap = cand_cap;
+        a.keep_pruned = p.keep_pruned ? 1u : 0u;
+        a.cand_keys = bs.cand_keys;
+        a.cand_cnt = bs.cand_cnt;
+        a.pairs = bs.pairs;
+        a.work.status = bs.status;
+        a.work.fail_count = &bs.ctrl->insert.fail_count;
+        a.work.fail_list = bs.fail_list;
+        a.sorted_pairs = bs.sorted;
+        a.seg_start = bs.seg_start;
+        a.n_seg = &bs.ctrl->n_seg;
+        return IDB_OK;
+    }
+
+    // Inserts PointIds [g0, g0 + b) on `layer`.  IDB_ERR_CAPACITY: an insert overflowed even the retry pass (with ka_first, before
+    // any row of this batch was written).
+    idb_status run(uint64_t g0, uint64_t b, uint32_t layer) {
+        cudaStream_t st = ix->stream;
+        const uint32_t cap = 2 * ix->M, efc = a.efc;
+        a.base = (uint32_t)g0;
+        a.count = (uint32_t)b;
+        a.work.n_work = b;
+        a.layer = layer;
+        a.n_pairs_cap = (uint32_t)(b * cap);
+        CUDA_TRY(cudaMemsetAsync(bs.ctrl, 0, sizeof(BuildCtrl), st));
+        // KA: descent of every insert, then (device-side, normally a no-op) a retry pass with 2^18-slot hash sets and 64k-entry
+        // tie lists for the inserts whose per-warp structures overflowed (e.g. inside a cluster of thousands of duplicate vectors)
+        BuildLaunch l;
+        l.op = kOpInsertSearch;
+        l.row_t = (int)((cap + 31) / 32);
+        l.ef_t = (int)((efc + 31) / 32);
+        l.stage = stage;
+        l.smem_per_warp = k2_smem;
+        l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kSearchWarps - 1) / kSearchWarps, (uint64_t)ix->search_grid()));
+        {
+            std::lock_guard<std::mutex> lk(ix->ctx->mu);  // the pool's tables must not be regrown under these launches
+            idb_status ts = ix->select_visited_tier(efc, a.tier, l.win);
+            if (ts == IDB_OK) ts = ix->attach_window(ix->lanes[0], l.win);
+            if (ts != IDB_OK) return ts;
+            a.work.work_counter = &bs.ctrl->insert.work_counter;
+            CUDA_TRY(build_dispatch_any(a, l, st));
+            BuildLaunch lr = l;
+            lr.grid = kRetryCtas;
+            lr.win = LaunchWindow();
+            BuildArgs r = retry_pass(a, *ix->ctx, &bs.ctrl->retry);
+            if (ix->retry_slots_override) {  // tests: a retry pass that can fail (with IDB_VIS_SLOTS, on ordinary data)
+                r.tier.gslots = ix->retry_slots_override;
+                r.tier.gshift = 32 - (uint32_t)std::log2((double)ix->retry_slots_override);
+            }
+            CUDA_TRY(build_dispatch_any(r, lr, st));
+        }
+        const int ka_b16 = a.tier.mode == kVisB16 ? ix->b16_level : 0;
+        if (ka_first) {
+            CUDA_TRY(cudaMemcpyAsync(bs.h_ctrl, bs.ctrl, sizeof(BuildCtrl), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            if (bs.h_ctrl->retry.fail_count)
+                return fail(IDB_ERR_CAPACITY, "%u inserts overflowed an internal per-insert structure (visited table / tie list) in the batch starting at %llu",
+                            bs.h_ctrl->retry.fail_count, (unsigned long long)g0);
+        }
+        // K2: neighbour selection for the new nodes, own rows, link requests
+        if (heuristic) {
+            l.op = kOpSelectNew;
+            l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
+            CUDA_TRY(build_dispatch_any(a, l, st));
+        } else {
+            select_simple_kernel<<<(unsigned)std::min<uint64_t>(b, 1024), 64, 0, st>>>(a);
+            CUDA_TRY(cudaGetLastError());
+        }
+        // group the link requests by target row
+        size_t tmp = bs.cub_bytes;
+        CUDA_TRY(cub::DeviceRadixSort::SortKeys(bs.cub_tmp, tmp, bs.pairs, bs.sorted, (int)(b * cap), 0, 64, st));
+        segment_heads_kernel<<<(unsigned)((b * cap + 255) / 256), 256, 0, st>>>(bs.sorted, (uint32_t)(b * cap), bs.seg_start,
+                                                                              &bs.ctrl->n_seg);
+        CUDA_TRY(cudaGetLastError());
+        // K2': re-prune every target row once
+        l.op = heuristic ? kOpRelink : kOpRelinkSimple;
+        l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b * cap + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
+        a.work.work_counter = &bs.ctrl->relink_work;
+        CUDA_TRY(build_dispatch_any(a, l, st));
+        if (!ka_first) {
+            CUDA_TRY(cudaMemcpyAsync(bs.h_ctrl, bs.ctrl, sizeof(BuildCtrl), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));  // fail fast: an insert that overflowed even the retry pass ends the build here
+            if (bs.h_ctrl->retry.fail_count)
+                return fail(IDB_ERR_CAPACITY, "%u inserts overflowed an internal per-insert structure (visited table / tie list) in the batch ending at %llu",
+                            bs.h_ctrl->retry.fail_count, (unsigned long long)(g0 + b));
+        }
+        ix->note_overflows(efc, b, bs.h_ctrl->insert.fail_count, ka_b16);  // too many b16 overflows: later batches use a larger flavour
+        return IDB_OK;
+    }
+};
+
 }  // namespace
 
 idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, const idb_params& p, uint32_t* out_ids) {
@@ -169,7 +319,10 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     ix->M = M;
     ix->ef_search = p.ef_search;
     ix->nchunks = (dim + 3) / 4;
-    if (n == 0) return IDB_OK;  // lib.rs:224-234
+    if (n == 0) {  // lib.rs:224-234; the storage is recorded for the rows a later insert adds
+        ix->bf16 = p.storage == IDB_STORAGE_BF16;
+        return IDB_OK;
+    }
     cudaStream_t st = ix->stream;
     const uint32_t cap = 2 * M;
     const size_t stride = (size_t)ix->nchunks * 4;
@@ -195,6 +348,7 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
         float* d_rows = nullptr;
         uint32_t* d_order = nullptr;
         CUDA_TRY(cudaMalloc(&ix->d_points, n * stride * sizeof(float)));
+        ix->cap = n;
         CUDA_TRY(cudaMalloc(&d_rows, n * (size_t)dim * sizeof(float)));
         CUDA_TRY(cudaMalloc(&d_order, n * sizeof(uint32_t)));
         CUDA_TRY(cudaMemcpyAsync(d_rows, rows, n * (size_t)dim * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -226,56 +380,11 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     if (top) CUDA_TRY(cudaMemcpyAsync(ix->d_upper_ptrs, ptrs.data(), top * sizeof(uint32_t*), cudaMemcpyHostToDevice, st));
 
     // ---- batch schedule + scratch -------------------------------------------------------------------------------
-    const uint32_t efc = p.ef_construction;
-    // Defaults: batch <= 16384 and <= 1/8 of the graph keeps recall@10 of the built graph close to the reference algorithm's own
-    // graph (tests/test_gpu_build.py checks it) while giving each batch enough inserts to fill the device.
-    uint32_t max_batch = p.insert_batch ? p.insert_batch : 16384u;
-    uint32_t growth = 8;  // a batch never exceeds 1/8 of the graph it is inserted into
-    if (!p.insert_batch) {  // tuning knobs for experiments (results stay valid HNSW graphs; determinism per setting)
-        if (const char* e = std::getenv("IDB_BUILD_MAXBATCH")) max_batch = (uint32_t)std::max(1, std::atoi(e));
-        if (const char* e = std::getenv("IDB_BUILD_GROWTH")) growth = (uint32_t)std::max(1, std::atoi(e));
-    }
-    const uint32_t cand_cap = std::max<uint32_t>((efc + 31) / 32 * 32, cap + kNewCap);
-    BuildScratch bs;
-    CUDA_TRY(cudaMalloc(&bs.cand_keys, (size_t)max_batch * cand_cap * 8));
-    CUDA_TRY(cudaMalloc(&bs.cand_cnt, (size_t)max_batch * 4));
-    CUDA_TRY(cudaMalloc(&bs.pairs, (size_t)max_batch * cap * 8));
-    CUDA_TRY(cudaMalloc(&bs.sorted, (size_t)max_batch * cap * 8));
-    CUDA_TRY(cudaMalloc(&bs.seg_start, (size_t)max_batch * cap * 4));
-    CUDA_TRY(cudaMalloc(&bs.status, (size_t)max_batch * 4));
-    CUDA_TRY(cudaMalloc(&bs.fail_list, (size_t)max_batch * 4));
-    CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&bs.h_ctrl), sizeof(BuildCtrl), cudaHostAllocDefault));
-    CUDA_TRY(cudaMalloc(&bs.ctrl, sizeof(BuildCtrl)));
-    CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, bs.cub_bytes, bs.pairs, bs.sorted, (int)(max_batch * cap), 0, 64, st));
-    CUDA_TRY(cudaMalloc(&bs.cub_tmp, std::max<size_t>(bs.cub_bytes, 16)));
-
-    // Staging the kept rows in shared memory (72 KB per 2-warp CTA -> 6 warps per SM) trades 32 resident warps for 6 to save reads
-    // that L1/L2 serve anyway, so it is off unless asked for.
-    bool stage = false;
-    if (const char* e = std::getenv("IDB_BUILD_STAGE")) stage = std::atoi(e) != 0 && SelectSmem::bytes(cand_cap, M, ix->nchunks, true) <= 56 * 1024;
-    const uint32_t k2_smem = (uint32_t)SelectSmem::bytes(cand_cap, M, ix->nchunks, stage);
-    // K2 / K2' are persistent grids of 2-warp CTAs.  They are issue-bound (pairwise distances on L1/L2-resident rows), so the grid
-    // asks for as many CTAs per SM as shared memory (228 KB per SM on an H100) and registers allow, up to 16 (32 warps per SM).
-    int k2_ctas_per_sm = (int)std::min<uint64_t>(16, std::max<uint64_t>(1, (200 * 1024) / std::max<uint32_t>(1, k2_smem * kBuildWarps)));
-    if (const char* e = std::getenv("IDB_BUILD_CTAS")) k2_ctas_per_sm = std::max(1, std::atoi(e));
-
-    BuildArgs a;
-    std::memset(&a, 0, sizeof(a));
-    a.g = ix->view();
-    a.g.n_upper = top;
-    a.zero = ix->d_zero;
-    a.efc = efc;
-    a.cand_cap = cand_cap;
-    a.keep_pruned = p.keep_pruned ? 1u : 0u;
-    a.cand_keys = bs.cand_keys;
-    a.cand_cnt = bs.cand_cnt;
-    a.pairs = bs.pairs;
-    a.work.status = bs.status;
-    a.work.fail_count = &bs.ctrl->insert.fail_count;
-    a.work.fail_list = bs.fail_list;
-    a.sorted_pairs = bs.sorted;
-    a.seg_start = bs.seg_start;
-    a.n_seg = &bs.ctrl->n_seg;
+    uint32_t max_batch = 0, growth = 0;
+    batch_schedule(p, &max_batch, &growth);
+    BatchRunner run;
+    idb_status rs = run.init(ix, p, max_batch, false);
+    if (rs != IDB_OK) return rs;
 
     for (uint32_t li = 0; li < num_layers; ++li) {  // lib.rs:304-329
         const uint32_t layer = num_layers - li - 1;
@@ -286,61 +395,9 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
             uint64_t b = 1;
             if (layer != top && max_batch > 1) b = std::min<uint64_t>(max_batch, std::max<uint64_t>(1, g0 / growth));
             b = std::min<uint64_t>(b, end - g0);
-            a.base = (uint32_t)g0;
-            a.count = (uint32_t)b;
-            a.work.n_work = b;
-            a.layer = layer;
-            a.n_pairs_cap = (uint32_t)(b * cap);
-            CUDA_TRY(cudaMemsetAsync(bs.ctrl, 0, sizeof(BuildCtrl), st));
-            // KA: descent of every insert, then (device-side, normally a no-op) a retry pass with 2^18-slot hash sets and 64k-entry
-            // tie lists for the inserts whose per-warp structures overflowed (e.g. inside a cluster of thousands of duplicate vectors)
-            BuildLaunch l;
-            l.op = kOpInsertSearch;
-            l.row_t = (int)((cap + 31) / 32);
-            l.ef_t = (int)((efc + 31) / 32);
-            l.stage = stage;
-            l.smem_per_warp = k2_smem;
-            l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kSearchWarps - 1) / kSearchWarps, (uint64_t)ix->search_grid()));
-            {
-                std::lock_guard<std::mutex> lk(ix->ctx->mu);  // the pool's tables must not be regrown under these launches
-                idb_status ts = ix->select_visited_tier(efc, a.tier, l.win);
-                if (ts == IDB_OK) ts = ix->attach_window(ix->lanes[0], l.win);
-                if (ts != IDB_OK) return ts;
-                a.work.work_counter = &bs.ctrl->insert.work_counter;
-                CUDA_TRY(build_dispatch_any(a, l, st));
-                BuildLaunch lr = l;
-                lr.grid = kRetryCtas;
-                lr.win = LaunchWindow();
-                CUDA_TRY(build_dispatch_any(retry_pass(a, *ix->ctx, &bs.ctrl->retry), lr, st));
-            }
-            const int ka_b16 = a.tier.mode == kVisB16 ? ix->b16_level : 0;
-            // K2: neighbour selection for the new nodes, own rows, link requests
-            if (p.heuristic) {
-                l.op = kOpSelectNew;
-                l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
-                CUDA_TRY(build_dispatch_any(a, l, st));
-            } else {
-                select_simple_kernel<<<(unsigned)std::min<uint64_t>(b, 1024), 64, 0, st>>>(a);
-                CUDA_TRY(cudaGetLastError());
-            }
-            // group the link requests by target row
-            size_t tmp = bs.cub_bytes;
-            CUDA_TRY(cub::DeviceRadixSort::SortKeys(bs.cub_tmp, tmp, bs.pairs, bs.sorted, (int)(b * cap), 0, 64, st));
-            segment_heads_kernel<<<(unsigned)((b * cap + 255) / 256), 256, 0, st>>>(bs.sorted, (uint32_t)(b * cap), bs.seg_start,
-                                                                                  &bs.ctrl->n_seg);
-            CUDA_TRY(cudaGetLastError());
-            // K2': re-prune every target row once
-            l.op = p.heuristic ? kOpRelink : kOpRelinkSimple;
-            l.grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((b * cap + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * k2_ctas_per_sm));
-            a.work.work_counter = &bs.ctrl->relink_work;
-            CUDA_TRY(build_dispatch_any(a, l, st));
-            CUDA_TRY(cudaMemcpyAsync(bs.h_ctrl, bs.ctrl, sizeof(BuildCtrl), cudaMemcpyDeviceToHost, st));
+            rs = run.run(g0, b, layer);
+            if (rs != IDB_OK) return rs;
             g0 += b;
-            CUDA_TRY(cudaStreamSynchronize(st));  // fail fast: an insert that overflowed even the retry pass ends the build here
-            if (bs.h_ctrl->retry.fail_count)
-                return fail(IDB_ERR_CAPACITY, "%u inserts overflowed an internal per-insert structure (visited table / tie list) in the batch ending at %llu",
-                            bs.h_ctrl->retry.fail_count, (unsigned long long)g0);
-            ix->note_overflows(efc, b, bs.h_ctrl->insert.fail_count, ka_b16);  // too many b16 overflows: later batches use a larger flavour
             if (p.progress) p.progress(g0, n, p.progress_user);  // set_position (core:519-525)
         }
         if (layer != 0) {  // lib.rs:323-328
@@ -351,6 +408,49 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     CUDA_TRY(cudaStreamSynchronize(st));
     if (p.progress) p.progress(n, n, p.progress_user);  // finish (core:331-334)
     return IDB_OK;
+}
+
+// Construction::insert(new, 0, layers) (core:437-528) for PointIds [n0, n0 + m), in the build's layer-0 batch schedule from g0 = n0
+// (also when the index has no upper layer, where the build inserts sequentially).  The caller holds the index exclusively and has
+// checked the arguments.  Rows: m x dim host floats, stored as the build stores them (zero padded, normalised for a cosine index,
+// then narrowed for a bf16 one).  global_ids: appended to the id map when the index has one.
+idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_params& p, const uint32_t* global_ids, uint32_t* out_ids) {
+    const uint64_t n0 = ix->n, n1 = n0 + m;
+    if (out_ids)
+        for (uint64_t i = 0; i < m; ++i) out_ids[i] = (uint32_t)(n0 + i);
+    if (m == 0) return IDB_OK;
+    // ---- storage: grow (copying the first n0 rows), then stage the new rows behind them; nothing below n0 changes -------------
+    idb_status s = ix->reserve_rows(n1);
+    if (s == IDB_OK) s = ix->stage_rows(rows, n0, m, global_ids);
+    if (s != IDB_OK) return s;
+    uint32_t max_batch = 0, growth = 0;
+    batch_schedule(p, &max_batch, &growth);
+    const uint64_t start = std::max<uint64_t>(n0, 1);  // an empty index: PointId 0 is the entry point (lib.rs:304-308)
+    BatchRunner run;
+    ix->n = n1;  // the traversals' view: every row the insert can reach
+    s = run.init(ix, p, std::min<uint64_t>(max_batch, n1 - start + 1), true);
+    if (s != IDB_OK) {
+        ix->n = n0;
+        return s;
+    }
+    // ---- layer 0, batched from n0 ---------------------------------------------------------------------------------------------
+    uint64_t reported = 0;  // the last progress value: the callback sees m exactly once
+    for (uint64_t g0 = start; g0 < n1;) {
+        const uint64_t b = std::min<uint64_t>(std::min<uint64_t>(max_batch, std::max<uint64_t>(1, g0 / growth)), n1 - g0);
+        s = run.run(g0, b, 0);
+        if (s == IDB_ERR_CAPACITY) {  // the batches before it stand; its rows were never written
+            ix->n = g0;
+            idb_status c = ix->build_codes();
+            return c == IDB_OK ? s : c;
+        }
+        if (s != IDB_OK) return s;
+        g0 += b;
+        reported = g0 - n0;
+        if (p.progress) p.progress(reported, m, p.progress_user);
+    }
+    CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    if (p.progress && reported != m) p.progress(m, m, p.progress_user);  // no batch ran: an empty index given one row
+    return ix->build_codes();  // from all stored rows: the table's step, offsets and error bound follow the new rows
 }
 
 }  // namespace idb
@@ -393,4 +493,38 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
     if (st != IDB_OK) { delete ix; return st; }
     *out_index = reinterpret_cast<idb_index*>(ix);
     return IDB_OK;
+}
+
+extern "C" idb_status idb_index_insert_f32(idb_index* index, const float* rows, uint64_t m, uint32_t dim, const idb_params* params,
+                                           const uint32_t* global_ids, uint32_t* out_ids) {
+    // checks that need neither the handle nor a device first, as the search entries do
+    if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
+    if (!params) return fail(IDB_ERR_INVALID_ARG, "params is null");
+    if (m && !rows) return fail(IDB_ERR_INVALID_ARG, "rows is null");
+    if (params->ef_construction == 0 || params->ef_construction > 1024)
+        return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", params->ef_construction);
+    if (params->heuristic && params->extend_candidates)
+        return fail(IDB_ERR_UNSUPPORTED,
+                    "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "
+                    "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns");
+    idb_status st = require_device();
+    if (st != IDB_OK) return st;
+    Index* ix = reinterpret_cast<Index*>(index);
+    // &mut self: no search, export or other insert runs while the index changes.  Every lane is taken (searches on other threads
+    // wait) and drained, so each search sees the index before or after this call.
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (auto& ln : ix->lanes) ln.mu.lock();
+    struct Unlock {
+        Index* ix;
+        ~Unlock() { for (auto& ln : ix->lanes) ln.mu.unlock(); }
+    } unlock{ix};
+    if (dim != ix->dim) return fail(IDB_ERR_INVALID_ARG, "dim %u differs from the index's %u", dim, ix->dim);
+    if (params->M != ix->M) return fail(IDB_ERR_INVALID_ARG, "M = %u differs from the index's %u", params->M, ix->M);
+    if (m && ix->d_id_map && !global_ids) return fail(IDB_ERR_INVALID_ARG, "the index has an id map: global_ids is required");
+    if (!ix->d_id_map && global_ids) return fail(IDB_ERR_INVALID_ARG, "global_ids given, but the index has no id map");
+    if (ix->n + m >= 0xFFFFFFFFull)
+        return fail(IDB_ERR_INVALID_ARG, "N = %llu + %llu >= u32::MAX (lib.rs:256)", (unsigned long long)ix->n, (unsigned long long)m);
+    CUDA_TRY(cudaSetDevice(ix->device));
+    for (auto& ln : ix->lanes) CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    return insert_index(ix, rows, m, *params, global_ids, out_ids);
 }

@@ -204,17 +204,18 @@ struct Index {
     std::atomic<uint32_t> next_lane{0};        // host-API calls rotate over the lanes
     std::atomic<int> last_lane{0};
 
-    uint64_t n = 0;
+    std::atomic<uint64_t> n{0};                // written by an insert while other threads may read it (searches take a lane first)
+    uint64_t cap = 0;                          // rows allocated for points, zero and the id map (>= n; grows by doubling on insert)
     uint32_t dim = 0, nchunks = 0, M = 32, ef_search = 100;
-    float* d_points = nullptr;                 // n x nchunks*4 f32 (PointId order); null when the rows are stored as bf16
-    uint16_t* d_points_bf16 = nullptr;         // n x nchunks*4 bf16 (storage = IDB_STORAGE_BF16)
+    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored as bf16
+    uint16_t* d_points_bf16 = nullptr;         // cap x nchunks*4 bf16 (storage = IDB_STORAGE_BF16)
     bool bf16 = false;
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
-    uint32_t* d_zero = nullptr;                // n x 2M
+    uint32_t* d_zero = nullptr;                // cap x 2M (rows past n: INVALID)
     std::vector<uint32_t*> d_upper;            // [l-1] -> n_l x M
     std::vector<uint64_t> upper_n;
     const uint32_t** d_upper_ptrs = nullptr;   // device copy of the pointer table
-    uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map)
+    uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map), cap entries
     bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
     // Screening table of the stored rows (DESIGN §2, §4): n x nchunks u32 of 8-bit codes + 3 x nchunks float4 (scale, offset, E),
     // one code step for every element and the bound on every row's coding error (GraphView::cstep / cerr).
@@ -230,6 +231,7 @@ struct Index {
     uint32_t vis_mult = 4;        // hash flavour: slots = next_pow2(vis_mult * 2M * ef): load <= ~0.15, probe chains ~1
     uint32_t vis_slots_override = 0; // IDB_VIS_SLOTS (tests): exact hash-table size, to force the overflow -> retry path
     uint32_t b16_bytes_override = 0; // IDB_B16_BYTES (tests / sweeps): exact b16 table bytes per warp in use
+    uint32_t retry_slots_override = 0; // IDB_RETRY_SLOTS (tests): hash slots of the build's and the insert's KA retry pass
     uint32_t b16_cap_16ths = 11;     // IDB_B16_CAP (tests): hand a query to the retry pass beyond this many sixteenths of the slots
     int vis_tier = -1;            // IDB_VIS_TIER: -1 auto (b16 when exact for this n, else bitmap / hash), 0 hash, 1 bitmap, 2 b16
     int variant = 0;              // IDB_VARIANT: alternative (rows in flight, CTAs/SM) instantiations of K1
@@ -248,6 +250,12 @@ struct Index {
                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
     idb_status narrow_points_to_bf16();                                  // d_points (f32) -> d_points_bf16, frees d_points
+    // Storage for at least `rows` points: points, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
+    // n rows.  Everything is allocated before anything is freed, so a failure leaves the index as it was.
+    idb_status reserve_rows(uint64_t rows);
+    // Rows [r0, r0 + m) (r0 >= n, within cap) from m x dim host floats, as the build stores them: zero padded, normalised for a
+    // cosine index, narrowed for a bf16 one; their zero rows INVALID; global_ids (m entries) into the id map when it exists.
+    idb_status stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids);
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
     int search_grid() const;

@@ -117,7 +117,7 @@ idb_status idb_index_set_id_map(idb_index* index, const uint32_t* global_ids) {
         return IDB_OK;
     }
     if (ix->n == 0) return IDB_OK;
-    if (!ix->d_id_map) CUDA_TRY(cudaMalloc(&ix->d_id_map, ix->n * 4));
+    if (!ix->d_id_map) CUDA_TRY(cudaMalloc(&ix->d_id_map, ix->cap * 4));
     CUDA_TRY(cudaMemcpyAsync(ix->d_id_map, global_ids, ix->n * 4, cudaMemcpyHostToDevice, ix->stream));
     CUDA_TRY(cudaStreamSynchronize(ix->stream));
     return IDB_OK;

@@ -8,6 +8,8 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
   * `Hnsw.search_many / HnswMap.search_many` expose the batched search the GPU is built for;
   * `Hnsw.search_exact / HnswMap.search_exact` return the exact k nearest points (a scan of every point, ties by lower PointId),
     the ground truth to tune `ef_search` against;
+  * `Hnsw.insert / HnswMap.insert` append points to a built or loaded index (layer 0 only, PointIds continue from the current
+    count; DESIGN.md §6);
   * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
     DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it.
 """
@@ -127,6 +129,31 @@ class Hnsw:
         q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
         return self._ix.exact_search(q, k=k)
 
+    def _insert(self, points, config, on_partial=None):
+        """on_partial(k): called before an IdbError propagates, with how many of the points the index kept (an insert that fails
+        with ERR_CAPACITY keeps the batches before the failing one)."""
+        m = _to_matrix(points, self._dim)
+        config = Config() if config is None else config
+        kw = dict(ef_construction=config.ef_construction)
+        if config.heuristic is None:
+            kw["heuristic"] = 0
+        else:
+            kw.update(heuristic=1, extend_candidates=int(bool(config.heuristic.extend_candidates)),
+                      keep_pruned=int(bool(config.heuristic.keep_pruned)))
+        n0 = int(self._ix.info().n)
+        try:
+            return [int(i) for i in self._ix.insert(m, **kw)]
+        except _abi.IdbError:
+            if on_partial is not None:
+                on_partial(int(self._ix.info().n) - n0)
+            raise
+
+    def insert(self, points, config=None):
+        """Not in the reference module: adds points to the index and returns their PointIds (the current count onwards, in order).
+        Construction::insert on layer 0 (the upper layers keep sampling the points the index was built with).  config supplies
+        ef_construction and the heuristic (None: Config() defaults); points are zero-padded to the index's dimension."""
+        return self._insert(points, config)
+
     def dump(self, fname):
         """py:131-137: bincode layout of `Hnsw` (ef_search, points, zero, layers)."""
         self._ix.save(fname)
@@ -155,6 +182,17 @@ class HnswMap(Hnsw):
         for orig, pid in enumerate(ids):
             by_pid[int(pid)] = vals[orig]
         return HnswMap(ix, by_pid)
+
+    def insert(self, points, values, config=None):
+        """Hnsw.insert, with one value per point; values follow the new PointIds (and `dump` writes them).  If the insert fails
+        with ERR_CAPACITY, the values of the points the index kept are appended before the error propagates."""
+        vals = [str(v) if not isinstance(v, str) else v for v in values]
+        if len(vals) != len(points):
+            raise ValueError("one value per point")
+        # values follow PointIds, also for the points a failed insert kept
+        ids = self._insert(points, config, on_partial=lambda kept: self._values.extend(vals[:kept]))
+        self._values.extend(vals)
+        return ids
 
     @property
     def values(self):

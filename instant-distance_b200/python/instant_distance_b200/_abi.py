@@ -25,7 +25,7 @@ SYMBOLS = [
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
-    "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane",
+    "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32",
 ]
 
 
@@ -73,6 +73,7 @@ def lib():
     L.idb_index_from_graph_ex.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_uint32,
                                           C.POINTER(u32p), u64p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp)]
     L.idb_index_load_ex.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
+    L.idb_index_insert_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), u32p, u32p]
     L.idb_normalize_f32.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_int32, f32p]
     L.idb_index_metric.argtypes = [vp, u32p]
     L.idb_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.c_uint32, u32p, f32p, u32p]
@@ -211,6 +212,30 @@ class Index:
         h = C.c_void_p()
         check(lib().idb_build_ex(ptr(rows, C.c_float), n, dim, C.byref(p), _metric(metric), C.byref(h), ptr(ids, C.c_uint32)))
         return cls(h), ids
+
+    def insert(self, rows, global_ids=None, progress=None, **kw):
+        """Appends rows (m x dim) to the index on layer 0 (idb_index_insert_f32); returns their PointIds, n0 .. n0+m-1.
+        kw: idb_params fields (ef_construction, heuristic, keep_pruned, insert_batch; M defaults to the index's).  global_ids: the
+        rows' entries for the id map, required when the index has one."""
+        rows = f32(rows)
+        if rows.ndim == 1:
+            rows = rows[None, :]
+        m, dim = rows.shape
+        kw.setdefault("M", int(self.info().M))
+        p = default_params(**kw)
+        cb = None
+        if progress is not None:
+            cb = PROGRESS_FN(lambda done, total, _user: progress(int(done), int(total)))
+            p.progress = C.cast(cb, C.c_void_p)
+        g = None
+        if global_ids is not None:
+            g = np.ascontiguousarray(global_ids, dtype=np.uint32)
+            if g.shape != (m,):
+                raise ValueError("global_ids must have one entry per row")
+        ids = np.empty(m, dtype=np.uint32)
+        check(lib().idb_index_insert_f32(self._h, ptr(rows, C.c_float), m, dim, C.byref(p), None if g is None else ptr(g, C.c_uint32),
+                                         ptr(ids, C.c_uint32)))
+        return ids
 
     def save(self, path):
         check(lib().idb_index_save(self._h, os.fsencode(path)))

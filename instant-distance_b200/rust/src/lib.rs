@@ -38,6 +38,7 @@ extern "C" {
     fn idb_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, ef: u32, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
     fn idb_exact_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
     fn idb_exact_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
+    fn idb_index_insert_f32(ix: *mut IdbIndex, rows: *const f32, m: u64, dim: u32, p: *const IdbParams, global_ids: *const u32, out_ids: *mut u32) -> i32;
     fn idb_index_free(ix: *mut IdbIndex);
     fn idb_last_error() -> *const c_char;
     // Batched / device-side / multi-GPU entry points (no counterpart in the reference; see include/instant_distance_b200.h):
