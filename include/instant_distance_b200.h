@@ -29,11 +29,15 @@ extern "C" {
 #define IDB_INVALID 0xFFFFFFFFu
 #define IDB_STORAGE_F32 0u
 #define IDB_STORAGE_BF16 1u
+/* fp16 rows (DESIGN.md §3b): rounded to nearest even, subnormals kept, +-0 / +-inf / NaN kept; 11 significant bits against bf16's 8,
+ * at the same 2 bytes per element.  A finite value that would round to +-inf (|x| >= 65520) is refused with IDB_ERR_INVALID_ARG,
+ * naming its row and element, before the index changes.  Widened exactly to f32 for every distance, export and save. */
+#define IDB_STORAGE_F16 2u
 /* Metrics (DESIGN.md §3a).  IDB_METRIC_COSINE: every row and every query is normalised in the canonical order (x / sqrt(sum x^2),
  * correctly rounded; a row whose sum of squares overflows becomes zeros and NaN), the traversal runs the canonical squared L2 on
  * the normalised rows, and the reported distance is half of it: 1 - cos(x, y) (0 .. 2).  An all-zero row stays zero, so it is at
- * 0.5 from every other row and at 0 from another zero row.  An index stores the normalised rows (bf16: normalised in f32, then
- * rounded) and exports / saves them. */
+ * 0.5 from every other row and at 0 from another zero row.  An index stores the normalised rows (bf16 / fp16: normalised in f32,
+ * then rounded) and exports / saves them. */
 #define IDB_METRIC_L2SQ 0u
 #define IDB_METRIC_COSINE 1u
 
@@ -72,8 +76,9 @@ typedef struct idb_params {
     uint32_t insert_batch;      /* GPU build: concurrent inserts per step (rayon's worker count in the
                                    reference, core:316-318).  0 = auto, 1 = strictly sequential order. */
     int32_t  device;            /* CUDA device ordinal */
-    uint32_t storage;           /* IDB_STORAGE_F32 (default) or IDB_STORAGE_BF16: rows rounded to bf16 (RNE) and kept in HBM at
-                                   half the bytes; distances still accumulate in fp32 in the same canonical order */
+    uint32_t storage;           /* IDB_STORAGE_F32 (default), IDB_STORAGE_BF16 or IDB_STORAGE_F16: rows rounded to bf16 / fp16 (RNE)
+                                   and kept in HBM at half the bytes; distances still accumulate in fp32 in the same canonical
+                                   order.  An index with no rows records it for the rows a later insert adds. */
     /* Builder::progress(ProgressBar) (core:70-75; feature `indicatif`): called on the building thread with the number of
      * points whose insertion has been enqueued so far (set_position, core:519-525) and the total (set_length, core:216-222);
      * the last call has done == total (finish, core:331-334).  NULL = no reporting. */
@@ -106,7 +111,9 @@ IDB_API idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, con
  *     insert_batch (1 = the sequential reference order), else IDB_BUILD_MAXBATCH / IDB_BUILD_GROWTH (defaults 16384 / 8).  Unlike
  *     the build, an index with no upper layer is also inserted into in batches.  An empty index (n0 = 0) makes the first row its
  *     entry point, PointId 0.
- *   - Rows are stored as the build stores them: zero padded, normalised for a cosine index, then narrowed for a bf16 one.
+ *   - Rows are stored as the build stores them: zero padded, normalised for a cosine index, then narrowed for a bf16 / fp16 one.
+ *     An fp16 index refuses rows with a finite value that rounds to infinity (IDB_ERR_INVALID_ARG, naming the row i of `rows` and
+ *     the element); the index's rows, graph and n stay as they were.
  *   - params: ef_construction (1..1024), heuristic, keep_pruned, insert_batch and progress (called with the rows inserted so far
  *     and m) are read; M must equal the index's M; extend_candidates is refused as by the build; seed, ml, ef_search, storage and
  *     device are ignored.  dim must equal the index's dim; n0 + m >= u32::MAX is refused (core:256); m = 0 does nothing.
@@ -136,9 +143,10 @@ IDB_API idb_status idb_index_from_graph_bf16(const float* points, uint64_t n, ui
                                      const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
                                      const uint64_t* upper_n, int32_t device, idb_index** out_index);
 
-/* Both of the above and the metric: storage = IDB_STORAGE_*, metric = IDB_METRIC_*.  With IDB_METRIC_COSINE the points are taken
- * as given (normalising is not idempotent bit for bit, so an adopted graph keeps the exact rows it was built on): every row must
- * be all zeros or have |sum x^2 - 1| <= 1e-2 (which lets bf16-rounded unit rows through), else IDB_ERR_INVALID_ARG.
+/* Both of the above and the metric: storage = IDB_STORAGE_* (IDB_STORAGE_F16: the rows rounded to fp16; results equal the reference
+ * algorithm run on the fp16-rounded points), metric = IDB_METRIC_*.  With IDB_METRIC_COSINE the points are taken as given
+ * (normalising is not idempotent bit for bit, so an adopted graph keeps the exact rows it was built on): every row must be all zeros
+ * or have |sum x^2 - 1| <= 1e-2 (which lets bf16- and fp16-rounded unit rows through), else IDB_ERR_INVALID_ARG.
  * idb_normalize_f32 gives the canonical normalisation. */
 IDB_API idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
                                            const uint32_t* zero, uint32_t n_upper, const uint32_t* const* upper,
@@ -146,7 +154,7 @@ IDB_API idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint
                                            idb_index** out_index);
 
 /* The canonical normalisation of n rows of dim f32 (DESIGN.md §3a) on the device: out (n x dim, host) = what a cosine index
- * stores for `rows` (before any bf16 rounding).  For callers preparing rows for idb_index_from_graph_ex, and for parity tests. */
+ * stores for `rows` (before any bf16 / fp16 rounding).  For callers preparing rows for idb_index_from_graph_ex, and for parity tests. */
 IDB_API idb_status idb_normalize_f32(const float* rows, uint64_t n, uint32_t dim, int32_t device, float* out);
 
 /* Hnsw::search(point, &mut Search) (core:352-383), batched: one independent search per query row.
@@ -207,9 +215,9 @@ IDB_API idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint
  * lane = 0xFFFFFFFF: the lane the last call on this index used. */
 IDB_API idb_status idb_last_search_full_fetches(idb_index* index, uint32_t lane, uint64_t* out_rows);
 /* Diagnostics: which instantiation of the search kernel the last call on `lane` launched (its main pass; the retry pass uses the same
- * one).  out (8 u32) = {CH (float4 chunks per lane of a row, 0 = the long-row kernel), ROW_T, EF_T, B (rows in flight per lane), 1 if the
- * rows are bf16, 1 if FULL (no chunk predicates), 1 if TMA, the IDB_VARIANT case taken (0 = the default dispatch)}; all zeros when
- * the last call launched no kernel.  lane = 0xFFFFFFFF: the lane the last call on this index used. */
+ * one).  out (8 u32) = {CH (float4 chunks per lane of a row, 0 = the long-row kernel), ROW_T, EF_T, B (rows in flight per lane), the
+ * row type (IDB_STORAGE_*: 0 f32, 1 bf16, 2 fp16), 1 if FULL (no chunk predicates), 1 if TMA, the IDB_VARIANT case taken (0 = the
+ * default dispatch; the variants exist for f32 rows only)}; all zeros when the last call launched no kernel.  lane = 0xFFFFFFFF: the lane the last call on this index used. */
 IDB_API idb_status idb_last_search_kernel(idb_index* index, uint32_t lane, uint32_t* out);
 /* enabled = 1: reserve persisting L2 for the visited tables on `device` (see idb_search_batch_f32).  enabled = 0 (the default):
  * this library never touches the device's persisting-L2 limit nor attaches access-policy windows on `device`. */
@@ -247,6 +255,11 @@ IDB_API idb_status idb_index_load(const char* path, uint32_t dim, uint32_t M, in
  * length nor all zeros: IDB_ERR_FORMAT). */
 IDB_API idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M, uint32_t metric, int32_t device, idb_index** out_index,
                                      uint64_t* out_values_offset);
+/* Same, stored as `storage` (IDB_STORAGE_*); idb_index_load_ex = IDB_STORAGE_F32.  The file always holds f32 rows (a bf16 or fp16
+ * index saves its rows widened, exactly), so saving an index and loading it with its own storage gives back the same rows.  Unknown
+ * storage: IDB_ERR_INVALID_ARG; IDB_STORAGE_F16 and a row value that rounds to infinity in fp16: IDB_ERR_INVALID_ARG. */
+IDB_API idb_status idb_index_load_storage(const char* path, uint32_t dim, uint32_t M, uint32_t metric, uint32_t storage, int32_t device,
+                                          idb_index** out_index, uint64_t* out_values_offset);
 
 /* Measurement hooks (bench.py): when enabled, CUDA events are recorded on the index stream immediately around the
  * dominant kernel of each call (K1 search_layer for searches); idb_index_last_kernel_ms waits for that kernel and

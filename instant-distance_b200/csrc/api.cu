@@ -78,7 +78,7 @@ cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, ui
     return cudaGetLastError();
 }
 
-// f32 -> bf16 (round to nearest even) and back (exact), element-wise over the padded row matrix
+// f32 -> bf16 / fp16 (round to nearest even) and back (exact), element-wise over the padded row matrix
 __global__ void narrow_bf16_kernel(const float* src, uint16_t* dst, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const uint32_t b = __float_as_uint(src[i]);
@@ -91,6 +91,34 @@ __global__ void narrow_bf16_kernel(const float* src, uint16_t* dst, size_t n) {
 __global__ void widen_bf16_kernel(const uint16_t* src, float* dst, size_t n) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
         dst[i] = __uint_as_float((uint32_t)src[i] << 16);
+}
+// cvt.rn.f16.f32 is RNE with subnormal results kept and overflow to +-inf (refused beforehand by check_f16_range); a NaN keeps its sign
+// and top payload bits, quieted (what the x86 F16C conversion and numpy give for a quiet NaN).
+__global__ void narrow_f16_kernel(const float* src, uint16_t* dst, size_t n) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const float x = src[i];
+        const uint32_t b = __float_as_uint(x);
+        unsigned short h;
+        if ((b & 0x7fffffffu) > 0x7f800000u) h = (unsigned short)(((b >> 16) & 0x8000u) | 0x7e00u | ((b >> 13) & 0x3ffu));
+        else asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
+        dst[i] = h;
+    }
+}
+// Exact, and a NaN keeps its sign and payload (cvt.f32.f16 would return the canonical NaN), so an export or a save gives back the
+// f32 value of every stored bit pattern.
+__global__ void widen_f16_kernel(const uint16_t* src, float* dst, size_t n) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t h = src[i];
+        dst[i] = (h & 0x7fffu) > 0x7c00u ? __uint_as_float(((h & 0x8000u) << 16) | 0x7f800000u | ((h & 0x3ffu) << 13))
+                                         : widen_f16x2(h).x;
+    }
+}
+// The smallest flat index of a finite element that rounds to +-inf in fp16 (|x| >= 65520, halfway to the next binade past 65504).
+__global__ void f16_overflow_kernel(const float* src, size_t n, unsigned long long* first) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const float x = fabsf(src[i]);
+        if (x >= 65520.f && x <= 3.402823466e38f) atomicMin(first, (unsigned long long)i);
+    }
 }
 
 // Adjacency sanity check for graphs adopted from outside (idb_index_from_graph_*, idb_index_load): every entry must be
@@ -670,16 +698,56 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, 
     return IDB_OK;
 }
 
-idb_status Index::narrow_points_to_bf16() {
+cudaError_t narrow_elems(const float* src, uint16_t* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    if (type == kRowF16) narrow_f16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
+    else narrow_bf16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
+    return cudaGetLastError();
+}
+cudaError_t widen_elems(const uint16_t* src, float* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    if (type == kRowF16) widen_f16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
+    else widen_bf16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
+    return cudaGetLastError();
+}
+
+idb_status check_f16_range(const float* d_rows, uint64_t m, uint32_t nchunks, const uint32_t* input_row, uint64_t row0, int num_sms,
+                           cudaStream_t st) {
+    const size_t stride = (size_t)nchunks * 4, total = m * stride;
+    if (total == 0) return IDB_OK;
+    unsigned long long* d_first = nullptr;
+    unsigned long long first = ~0ull;
+    CUDA_TRY(cudaMalloc(&d_first, 8));
+    cudaError_t e = cudaMemcpyAsync(d_first, &first, 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) {
+        f16_overflow_kernel<<<num_sms * 8, 256, 0, st>>>(d_rows, total, d_first);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&first, d_first, 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    float x = 0.f;
+    if (e == cudaSuccess && first != ~0ull) e = cudaMemcpy(&x, d_rows + first, 4, cudaMemcpyDeviceToHost);
+    cudaFree(d_first);
+    CUDA_TRY(e);
+    if (first == ~0ull) return IDB_OK;
+    const uint64_t r = first / stride;
+    return fail(IDB_ERR_INVALID_ARG, "fp16 storage: row %llu, element %llu is %g, which rounds to infinity in fp16 (|x| >= 65520)",
+                (unsigned long long)(input_row ? input_row[r] : row0 + r), (unsigned long long)(first % stride), (double)x);
+}
+
+idb_status Index::narrow_points(uint32_t type, const uint32_t* input_row) {
+    if (type == kRowF16) {
+        const idb_status s = check_f16_range(d_points, n, nchunks, input_row, 0, num_sms, stream);
+        if (s != IDB_OK) return s;
+    }
     const size_t total = n * (size_t)nchunks * 4;
-    if (total == 0) { bf16 = true; return IDB_OK; }
-    CUDA_TRY(cudaMalloc(&d_points_bf16, cap * (size_t)nchunks * 4 * 2));
-    narrow_bf16_kernel<<<num_sms * 8, 256, 0, stream>>>(d_points, d_points_bf16, total);
-    CUDA_TRY(cudaGetLastError());
+    if (total == 0) { row_type = type; return IDB_OK; }
+    CUDA_TRY(cudaMalloc(&d_points16, cap * (size_t)nchunks * 4 * 2));
+    CUDA_TRY(narrow_elems(d_points, d_points16, total, type, num_sms, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     cudaFree(d_points);
     d_points = nullptr;
-    bf16 = true;
+    row_type = type;
     return IDB_OK;
 }
 
@@ -690,12 +758,11 @@ idb_status Index::reserve_rows(uint64_t rows) {
     void* pts = nullptr;
     uint32_t* zero = nullptr;
     uint32_t* id_map = nullptr;
-    cudaError_t e = cudaMalloc(&pts, want * stride * (bf16 ? 2 : 4));
+    cudaError_t e = cudaMalloc(&pts, want * stride * elem_bytes());
     if (e == cudaSuccess) e = cudaMalloc(&zero, want * width * 4);
     if (e == cudaSuccess && d_id_map) e = cudaMalloc(&id_map, want * 4);
     if (e == cudaSuccess && n) {
-        e = cudaMemcpyAsync(pts, bf16 ? static_cast<const void*>(d_points_bf16) : static_cast<const void*>(d_points),
-                            n * stride * (bf16 ? 2 : 4), cudaMemcpyDeviceToDevice, stream);
+        e = cudaMemcpyAsync(pts, this->rows(), n * stride * elem_bytes(), cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(zero, d_zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(id_map, d_id_map, n * 4, cudaMemcpyDeviceToDevice, stream);
     }
@@ -707,11 +774,11 @@ idb_status Index::reserve_rows(uint64_t rows) {
         CUDA_TRY(e);
     }
     cudaFree(d_points);
-    cudaFree(d_points_bf16);
+    cudaFree(d_points16);
     cudaFree(d_zero);
     cudaFree(d_id_map);
-    d_points = bf16 ? nullptr : static_cast<float*>(pts);
-    d_points_bf16 = bf16 ? static_cast<uint16_t*>(pts) : nullptr;
+    d_points = row_type == kRowF32 ? static_cast<float*>(pts) : nullptr;
+    d_points16 = row_type == kRowF32 ? nullptr : static_cast<uint16_t*>(pts);
     d_zero = zero;
     d_id_map = id_map;
     cap = want;
@@ -725,12 +792,17 @@ idb_status Index::stage_rows(const float* rows, uint64_t r0, uint64_t m, const u
     cudaError_t e = cudaMemsetAsync(tmp, 0, m * stride * 4, stream);
     if (e == cudaSuccess) e = cudaMemcpy2DAsync(tmp, stride * 4, rows, dim * 4, dim * 4, m, cudaMemcpyHostToDevice, stream);
     if (e == cudaSuccess && metric == kMetricCosine) e = normalize_rows(tmp, stride, tmp, m, dim, nchunks, num_sms, stream);
-    if (e == cudaSuccess && bf16) {  // normalised first, then rounded, as the build does
-        narrow_bf16_kernel<<<num_sms * 8, 256, 0, stream>>>(tmp, d_points_bf16 + r0 * stride, m * stride);
-        e = cudaGetLastError();
-    } else if (e == cudaSuccess) {
-        e = cudaMemcpyAsync(d_points + r0 * stride, tmp, m * stride * 4, cudaMemcpyDeviceToDevice, stream);
+    if (e == cudaSuccess && row_type == kRowF16) {  // before anything of the index is written; rows named as the caller numbers them
+        const idb_status s = check_f16_range(tmp, m, nchunks, nullptr, 0, num_sms, stream);
+        if (s != IDB_OK) {
+            cudaFree(tmp);
+            return s;
+        }
     }
+    if (e == cudaSuccess && row_type != kRowF32)  // normalised first, then rounded, as the build does
+        e = narrow_elems(tmp, d_points16 + r0 * stride, m * stride, row_type, num_sms, stream);
+    else if (e == cudaSuccess)
+        e = cudaMemcpyAsync(d_points + r0 * stride, tmp, m * stride * 4, cudaMemcpyDeviceToDevice, stream);
     if (e == cudaSuccess) e = fill_u32(d_zero + r0 * 2 * M, m * 2 * M, kInvalid, stream);
     if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(d_id_map + r0, global_ids, m * 4, cudaMemcpyHostToDevice, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
@@ -742,15 +814,15 @@ idb_status Index::stage_rows(const float* rows, uint64_t r0, uint64_t m, const u
 idb_status Index::copy_points_f32(float* host_out, uint64_t r0, uint64_t m) {
     if (m == 0) return IDB_OK;
     const size_t stride = (size_t)nchunks * 4;
-    if (!bf16) {
+    if (row_type == kRowF32) {
         CUDA_TRY(cudaMemcpy2DAsync(host_out, dim * 4, d_points + r0 * stride, stride * 4, dim * 4, m, cudaMemcpyDeviceToHost, stream));
         CUDA_TRY(cudaStreamSynchronize(stream));
         return IDB_OK;
     }
     float* tmp = nullptr;
     CUDA_TRY(cudaMalloc(&tmp, m * stride * 4));
-    widen_bf16_kernel<<<num_sms * 8, 256, 0, stream>>>(d_points_bf16 + r0 * stride, tmp, m * stride);
-    cudaError_t e = cudaMemcpy2DAsync(host_out, dim * 4, tmp, stride * 4, dim * 4, m, cudaMemcpyDeviceToHost, stream);
+    cudaError_t e = widen_elems(d_points16 + r0 * stride, tmp, m * stride, row_type, num_sms, stream);
+    if (e == cudaSuccess) e = cudaMemcpy2DAsync(host_out, dim * 4, tmp, stride * 4, dim * 4, m, cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     cudaFree(tmp);
     CUDA_TRY(e);
@@ -759,8 +831,8 @@ idb_status Index::copy_points_f32(float* host_out, uint64_t r0, uint64_t m) {
 
 GraphView Index::view() const {
     GraphView g;
-    g.points = bf16 ? reinterpret_cast<const char*>(d_points_bf16) : reinterpret_cast<const char*>(d_points);
-    g.bf16 = bf16 ? 1u : 0u;
+    g.points = static_cast<const char*>(rows());
+    g.row_type = row_type;
     g.nchunks = nchunks;
     g.zero = d_zero;
     g.upper = d_upper_ptrs;
@@ -780,7 +852,7 @@ Index::~Index() {
     for (auto& ln : lanes)
         if (ln.stream) cudaStreamSynchronize(ln.stream);
     cudaFree(d_points);
-    cudaFree(d_points_bf16);
+    cudaFree(d_points16);
     cudaFree(d_codes);
     cudaFree(d_cparams);
     cudaFree(d_zero);
@@ -892,6 +964,57 @@ idb_status Index::upload(const float* points, uint64_t n_, uint32_t dim_, uint32
     return IDB_OK;
 }
 
+// idb_index_from_graph_ex.  from_file (idb_index_load_storage): a graph or row the checks refuse makes the file malformed
+// (IDB_ERR_FORMAT); rows beyond the range of the storage asked for stay IDB_ERR_INVALID_ARG, as for an adopted graph.
+idb_status adopt_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search, const uint32_t* zero,
+                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n, uint32_t storage, uint32_t metric,
+                       int32_t device, idb_index** out_index, bool from_file) {
+    if (!out_index) return fail(IDB_ERR_INVALID_ARG, "out_index is null");
+    *out_index = nullptr;
+    Index* ix = nullptr;
+    idb_status st = [&]() -> idb_status {
+        if (dim == 0) return fail(IDB_ERR_INVALID_ARG, "dim must be >= 1");
+        if (M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "M = %u unsupported (2..64)", M);
+        if (n >= 0xFFFFFFFFull) return fail(IDB_ERR_INVALID_ARG, "N = %llu >= u32::MAX (lib.rs:256)", (unsigned long long)n);
+        if (n && (!points || !zero)) return fail(IDB_ERR_INVALID_ARG, "points/zero is null");
+        if (n_upper > 31) return fail(IDB_ERR_INVALID_ARG, "too many layers");
+        if (n_upper && (!upper || !upper_n)) return fail(IDB_ERR_INVALID_ARG, "upper/upper_n is null");
+        if (storage > IDB_STORAGE_F16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
+        if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
+        if (metric == IDB_METRIC_COSINE) {
+            // Adopted rows are stored as given (normalising is not idempotent bit for bit), so they must already be unit rows; the
+            // tolerance lets bf16- and fp16-rounded unit rows through.
+            for (uint64_t r = 0; r < n; ++r) {
+                const float* x = points + r * dim;
+                double s = 0.0;
+                bool all_zero = true;
+                for (uint32_t i = 0; i < dim; ++i) {
+                    s += (double)x[i] * x[i];
+                    all_zero = all_zero && x[i] == 0.f;
+                }
+                if (!all_zero && !(std::fabs(s - 1.0) <= 1e-2))
+                    return fail(IDB_ERR_INVALID_ARG, "cosine index: row %llu has squared norm %g; rows must be unit length or all zeros "
+                                "(idb_normalize_f32 gives the canonical normalisation)", (unsigned long long)r, s);
+            }
+        }
+        ix = new (std::nothrow) Index();
+        if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
+        ix->metric = metric;
+        idb_status s = ix->init_device(device);
+        if (s == IDB_OK) s = ix->upload(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n);
+        return s;
+    }();
+    if (st == IDB_ERR_INVALID_ARG && from_file) st = IDB_ERR_FORMAT;
+    if (st == IDB_OK && storage != IDB_STORAGE_F32) st = ix->narrow_points(storage, nullptr);
+    if (st == IDB_OK) st = ix->build_codes();
+    if (st != IDB_OK) {
+        delete ix;
+        return st;
+    }
+    *out_index = reinterpret_cast<idb_index*>(ix);
+    return IDB_OK;
+}
+
 }  // namespace idb
 
 using namespace idb;
@@ -931,42 +1054,7 @@ idb_status idb_params_default(idb_params* p) {
 idb_status idb_index_from_graph_ex(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search, const uint32_t* zero,
                                    uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n, uint32_t storage,
                                    uint32_t metric, int32_t device, idb_index** out_index) {
-    if (!out_index) return fail(IDB_ERR_INVALID_ARG, "out_index is null");
-    *out_index = nullptr;
-    if (dim == 0) return fail(IDB_ERR_INVALID_ARG, "dim must be >= 1");
-    if (M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "M = %u unsupported (2..64)", M);
-    if (n >= 0xFFFFFFFFull) return fail(IDB_ERR_INVALID_ARG, "N = %llu >= u32::MAX (lib.rs:256)", (unsigned long long)n);
-    if (n && (!points || !zero)) return fail(IDB_ERR_INVALID_ARG, "points/zero is null");
-    if (n_upper > 31) return fail(IDB_ERR_INVALID_ARG, "too many layers");
-    if (n_upper && (!upper || !upper_n)) return fail(IDB_ERR_INVALID_ARG, "upper/upper_n is null");
-    if (storage != IDB_STORAGE_F32 && storage != IDB_STORAGE_BF16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
-    if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
-    if (metric == IDB_METRIC_COSINE) {
-        // Adopted rows are stored as given (normalising is not idempotent bit for bit), so they must already be unit rows; the
-        // tolerance lets bf16-rounded unit rows through.
-        for (uint64_t r = 0; r < n; ++r) {
-            const float* x = points + r * dim;
-            double s = 0.0;
-            bool all_zero = true;
-            for (uint32_t i = 0; i < dim; ++i) {
-                s += (double)x[i] * x[i];
-                all_zero = all_zero && x[i] == 0.f;
-            }
-            if (!all_zero && !(std::fabs(s - 1.0) <= 1e-2))
-                return fail(IDB_ERR_INVALID_ARG, "cosine index: row %llu has squared norm %g; rows must be unit length or all zeros "
-                            "(idb_normalize_f32 gives the canonical normalisation)", (unsigned long long)r, s);
-        }
-    }
-    auto* ix = new (std::nothrow) Index();
-    if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
-    ix->metric = metric;
-    idb_status st = ix->init_device(device);
-    if (st == IDB_OK) st = ix->upload(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n);
-    if (st == IDB_OK && storage == IDB_STORAGE_BF16) st = ix->narrow_points_to_bf16();
-    if (st == IDB_OK) st = ix->build_codes();
-    if (st != IDB_OK) { delete ix; return st; }
-    *out_index = reinterpret_cast<idb_index*>(ix);
-    return IDB_OK;
+    return adopt_graph(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n, storage, metric, device, out_index, false);
 }
 
 idb_status idb_index_from_graph_f32(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search,
@@ -1079,7 +1167,7 @@ idb_status idb_index_info(const idb_index* index, idb_info* out) {
     out->M = ix->M;
     out->ef_search = ix->ef_search;
     out->device = ix->device;
-    out->storage = ix->bf16 ? IDB_STORAGE_BF16 : IDB_STORAGE_F32;
+    out->storage = ix->row_type;
     out->n_layers = n == 0 ? 0 : (uint32_t)ix->d_upper.size() + 1;
     if (n) out->layer_n[0] = n;
     for (size_t l = 0; l < ix->upper_n.size() && l + 1 < 32; ++l) out->layer_n[l + 1] = ix->upper_n[l];

@@ -320,7 +320,7 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     ix->ef_search = p.ef_search;
     ix->nchunks = (dim + 3) / 4;
     if (n == 0) {  // lib.rs:224-234; the storage is recorded for the rows a later insert adds
-        ix->bf16 = p.storage == IDB_STORAGE_BF16;
+        ix->row_type = p.storage;
         return IDB_OK;
     }
     cudaStream_t st = ix->stream;
@@ -355,14 +355,14 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
         CUDA_TRY(cudaMemcpyAsync(d_order, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
         gather_rows_kernel<<<ix->num_sms * 8, 256, 0, st>>>(d_rows, d_order, ix->d_points, n, dim, (uint32_t)stride);
         CUDA_TRY(cudaGetLastError());
-        if (ix->metric == kMetricCosine)  // DESIGN §3a: a cosine index stores the normalised rows (bf16: normalised, then rounded)
+        if (ix->metric == kMetricCosine)  // DESIGN §3a: a cosine index stores the normalised rows (bf16 / fp16: normalised, then rounded)
             CUDA_TRY(normalize_rows(ix->d_points, stride, ix->d_points, n, dim, ix->nchunks, ix->num_sms, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         cudaFree(d_rows);
         cudaFree(d_order);
     }
-    if (p.storage == IDB_STORAGE_BF16) {
-        idb_status sb = ix->narrow_points_to_bf16();
+    if (p.storage != IDB_STORAGE_F32) {  // fp16: rows beyond its range are refused here, named by their input row
+        idb_status sb = ix->narrow_points(p.storage, order.data());
         if (sb != IDB_OK) return sb;
     }
     CUDA_TRY(cudaMalloc(&ix->d_zero, n * (size_t)cap * 4));
@@ -413,7 +413,8 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
 // Construction::insert(new, 0, layers) (core:437-528) for PointIds [n0, n0 + m), in the build's layer-0 batch schedule from g0 = n0
 // (also when the index has no upper layer, where the build inserts sequentially).  The caller holds the index exclusively and has
 // checked the arguments.  Rows: m x dim host floats, stored as the build stores them (zero padded, normalised for a cosine index,
-// then narrowed for a bf16 one).  global_ids: appended to the id map when the index has one.
+// then narrowed for a bf16 or fp16 one; fp16 rows beyond its range are refused before the index's rows or graph change).  global_ids:
+// appended to the id map when the index has one.
 idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_params& p, const uint32_t* global_ids, uint32_t* out_ids) {
     const uint64_t n0 = ix->n, n1 = n0 + m;
     if (out_ids)
@@ -476,7 +477,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
         return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", params->ef_construction);
     if (dim > 10240) return fail(IDB_ERR_UNSUPPORTED, "dim %u > 10240 is not supported (the owner row of a long-row traversal lives in shared memory)", dim);
     if (!(params->ml > 0.0f) || params->ml >= 1.0f) return fail(IDB_ERR_INVALID_ARG, "ml must be in (0, 1)");
-    if (params->storage != IDB_STORAGE_F32 && params->storage != IDB_STORAGE_BF16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
+    if (params->storage > IDB_STORAGE_F16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
     if (params->heuristic && params->extend_candidates)
         return fail(IDB_ERR_UNSUPPORTED,
                     "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "

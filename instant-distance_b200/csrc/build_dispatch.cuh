@@ -61,8 +61,7 @@ cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStre
 }
 template <int CH, int B, int NB>
 cudaError_t build_dispatch(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    if (a.g.bf16) return build_dispatch_rt<CH, B, NB, RowBF16>(a, l, st);
-    return build_dispatch_rt<CH, B, NB, RowF32>(a, l, st);
+    return with_row_type(a.g.row_type, [&](auto rt) { return build_dispatch_rt<CH, B, NB, decltype(rt)>(a, l, st); });
 }
 
 }  // namespace idb

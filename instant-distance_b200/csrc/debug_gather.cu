@@ -88,7 +88,7 @@ static idb_status gather_bench_impl(idb_index* index, uint32_t n_items, uint32_t
     if (!index || !out_ms) return fail(IDB_ERR_INVALID_ARG, "null argument");
     if (mode > 5 || atomics > 32) return fail(IDB_ERR_INVALID_ARG, "gather bench: mode 0..5, atomics <= 32");
     Index* ix = reinterpret_cast<Index*>(index);
-    if (ix->bf16 || ix->nchunks > 32 || ix->n == 0) return fail(IDB_ERR_UNSUPPORTED, "gather bench: f32 rows of <= 128 floats only");
+    if (ix->row_type != kRowF32 || ix->nchunks > 32 || ix->n == 0) return fail(IDB_ERR_UNSUPPORTED, "gather bench: f32 rows of <= 128 floats only");
     std::lock_guard<std::mutex> lk(ix->mu);
     CUDA_TRY(cudaSetDevice(ix->device));
     unsigned long long* d_counter = nullptr;

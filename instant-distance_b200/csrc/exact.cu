@@ -191,18 +191,18 @@ struct ScanChoice {
     int qw;
 };
 template <int CH>
-ScanChoice scan_choice(bool bf16) {
-    return ScanChoice{bf16 ? exact_scan_kernel<CH, RowBF16> : exact_scan_kernel<CH, RowF32>, ExactShape<CH>::QW};
+ScanChoice scan_choice(uint32_t row_type) {
+    return with_row_type(row_type, [](auto rt) { return ScanChoice{exact_scan_kernel<CH, decltype(rt)>, ExactShape<CH>::QW}; });
 }
-ScanChoice pick_scan(uint32_t nchunks, bool bf16) {
+ScanChoice pick_scan(uint32_t nchunks, uint32_t row_type) {
     switch (kernel_ch(nchunks)) {
-        case 1: return scan_choice<1>(bf16);
-        case 2: return scan_choice<2>(bf16);
-        case 3: return scan_choice<3>(bf16);
-        case 4: return scan_choice<4>(bf16);
-        case 6: return scan_choice<6>(bf16);
-        case 8: return scan_choice<8>(bf16);
-        default: return scan_choice<0>(bf16);
+        case 1: return scan_choice<1>(row_type);
+        case 2: return scan_choice<2>(row_type);
+        case 3: return scan_choice<3>(row_type);
+        case 4: return scan_choice<4>(row_type);
+        case 6: return scan_choice<6>(row_type);
+        case 8: return scan_choice<8>(row_type);
+        default: return scan_choice<0>(row_type);
     }
 }
 
@@ -225,7 +225,7 @@ static idb_status enqueue_exact(Index* ix, Lane& ln, const float* queries, bool 
     if (s == IDB_OK) s = ix->normalize_queries(ln, &qp, nq);
     if (s != IDB_OK) return s;
 
-    const ScanChoice sc = pick_scan(nchunks, ix->bf16);
+    const ScanChoice sc = pick_scan(nchunks, ix->row_type);
     int wpc = kExactWarps;
     size_t smem = 0;
     if (kernel_ch(nchunks) == 0) {  // one query per warp in shared memory: fewer warps per CTA for very long rows

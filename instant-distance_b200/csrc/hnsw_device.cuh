@@ -34,10 +34,13 @@ constexpr uint32_t kFullMask = 0xFFFFFFFFu;
 
 enum OptFlags : uint32_t { kOptPrefetchVectors = 1u, kOptPrefetchRows = 2u, kOptPrefetchNextRow = 8u };
 
+// How an index stores its rows; the values are the ABI's IDB_STORAGE_* (internal.cuh checks that).
+enum RowType : uint32_t { kRowF32 = 0, kRowBF16 = 1, kRowF16 = 2 };
+
 enum QueryStatus : uint32_t { kQueryOk = 0, kQueryVisitedOverflow = 1, kQueryTieOverflow = 2 };
 
 struct GraphView {
-    const char* points;          // n rows of nchunks 4-element chunks (dim rounded up to 4, zero padded); f32 (16 B/chunk) or bf16 (8 B/chunk)
+    const char* points;          // n rows of nchunks 4-element chunks (dim rounded up to 4, zero padded); f32 (16 B/chunk), bf16 or fp16 (8 B/chunk)
     uint32_t nchunks;            // 4-element chunks per row
     const uint32_t* zero;        // n x 2M
     const uint32_t* const* upper;  // device array: upper[l-1] = n_l x M
@@ -45,7 +48,7 @@ struct GraphView {
     uint32_t M;
     uint64_t n;
     uint32_t flags;              // kOpt* tuning switches (never change results)
-    uint32_t bf16;               // rows are stored as bf16 (BASELINE config 4's data format); arithmetic stays fp32
+    uint32_t row_type;           // RowType (= IDB_STORAGE_*): how the rows are stored; arithmetic stays fp32
     // Screening table (DESIGN §2, §4), or null: K1 then fetches every candidate row in full.
     const uint32_t* codes;       // n rows of nchunks u32: word c holds the 8-bit codes of elements 4c..4c+3 (byte k = element 4c+k)
     const float4* cparams;       // 3 x nchunks float4: per element scale, offset, E (x~ = fmaf(code, scale, offset), |x - x~| <= E)
@@ -77,10 +80,12 @@ __device__ __forceinline__ float lane_partial(const float4 (&q)[CH], const float
 }
 
 // Row storage types.  A lane always owns the same 4 ELEMENTS per 128-element block (chunk l, l+32, ...), so the canonical
-// fp32 summation order is the same for both; bf16 rows are widened exactly (bf16 -> f32 is a 16-bit shift).
-// `Raw` is what a lane keeps in registers while a batch of row loads is in flight (bf16 rows stay packed: half the
+// fp32 summation order is the same for all of them; bf16 and fp16 rows are widened exactly (bf16 -> f32 is a 16-bit shift, fp16 -> f32
+// is cvt.f32.f16, exact for every fp16 value, subnormals included).
+// `Raw` is what a lane keeps in registers while a batch of row loads is in flight (bf16 / fp16 rows stay packed: half the
 // registers per row, so twice as many rows in flight); widen() runs at the point of use.
 struct RowF32 {
+    static constexpr uint32_t kType = kRowF32;
     static constexpr uint32_t kChunkBytes = 16;
     using Raw = float4;
     static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
@@ -89,6 +94,7 @@ struct RowF32 {
     static __device__ __forceinline__ float4 ld(const char* p) { return ld_raw(p); }
 };
 struct RowBF16 {
+    static constexpr uint32_t kType = kRowBF16;
     static constexpr uint32_t kChunkBytes = 8;
     using Raw = uint2;
     static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
@@ -99,6 +105,33 @@ struct RowBF16 {
     }
     static __device__ __forceinline__ float4 ld(const char* p) { return widen(ld_raw(p)); }
 };
+// The two fp16 values packed in u (element 2i in the low half), widened exactly.
+__device__ __forceinline__ float2 widen_f16x2(uint32_t u) {
+    float2 f;
+    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\tcvt.f32.f16 %0, lo;\n\tcvt.f32.f16 %1, hi;\n\t}"
+        : "=f"(f.x), "=f"(f.y)
+        : "r"(u));
+    return f;
+}
+struct RowF16 {
+    static constexpr uint32_t kType = kRowF16;
+    static constexpr uint32_t kChunkBytes = 8;
+    using Raw = uint2;
+    static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
+    static __device__ __forceinline__ Raw zero() { return make_uint2(0u, 0u); }
+    static __device__ __forceinline__ float4 widen(Raw u) {
+        const float2 a = widen_f16x2(u.x), b = widen_f16x2(u.y);
+        return make_float4(a.x, a.y, b.x, b.y);
+    }
+    static __device__ __forceinline__ float4 ld(const char* p) { return widen(ld_raw(p)); }
+};
+// f(RT()) for the row type `row_type` of an index: the one place a run-time row type becomes a template argument.
+template <class F>
+auto with_row_type(uint32_t row_type, F&& f) {
+    if (row_type == kRowBF16) return f(RowBF16());
+    if (row_type == kRowF16) return f(RowF16());
+    return f(RowF32());
+}
 // This lane's CH chunks of row `pid` (zeros beyond the row's last chunk).
 template <int CH, class RT>
 __device__ __forceinline__ void load_row(const GraphView& g, uint32_t pid, int lane, float4 (&q)[CH]) {
@@ -144,7 +177,7 @@ __device__ __forceinline__ void q_from_f32(QVec<CH>& q, const float4* row, uint3
         }
     }
 }
-// q <- point row `pid` (f32 or bf16 storage)
+// q <- point row `pid` (any row type, widened)
 template <int CH, class RT>
 __device__ __forceinline__ void q_from_point(QVec<CH>& q, const GraphView& g, uint32_t pid, int lane) {
     if constexpr (CH == 0) {

@@ -189,7 +189,7 @@ struct Lane {
     uint64_t ctrl_nq = 0;
     uint64_t last_nq = 0;
     uint32_t last_launches = 0;
-    // the template arguments of the lane's last main K1 launch: {CH, ROW_T, EF_T, B, bf16 rows, FULL, TMA, IDB_VARIANT taken}
+    // the template arguments of the lane's last main K1 launch: {CH, ROW_T, EF_T, B, RowType, FULL, TMA, IDB_VARIANT taken}
     uint32_t last_kernel[8] = {};
     void free_all();
 };
@@ -207,9 +207,9 @@ struct Index {
     std::atomic<uint64_t> n{0};                // written by an insert while other threads may read it (searches take a lane first)
     uint64_t cap = 0;                          // rows allocated for points, zero and the id map (>= n; grows by doubling on insert)
     uint32_t dim = 0, nchunks = 0, M = 32, ef_search = 100;
-    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored as bf16
-    uint16_t* d_points_bf16 = nullptr;         // cap x nchunks*4 bf16 (storage = IDB_STORAGE_BF16)
-    bool bf16 = false;
+    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored in 2 bytes
+    uint16_t* d_points16 = nullptr;            // cap x nchunks*4 bf16 or fp16 (row_type kRowBF16 / kRowF16), else null
+    uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
     uint32_t* d_zero = nullptr;                // cap x 2M (rows past n: INVALID)
     std::vector<uint32_t*> d_upper;            // [l-1] -> n_l x M
@@ -249,12 +249,17 @@ struct Index {
     idb_status upload(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef, const uint32_t* zero,
                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
-    idb_status narrow_points_to_bf16();                                  // d_points (f32) -> d_points_bf16, frees d_points
+    uint32_t elem_bytes() const { return row_type == kRowF32 ? 4u : 2u; }
+    const void* rows() const { return row_type == kRowF32 ? static_cast<const void*>(d_points) : static_cast<const void*>(d_points16); }
+    // d_points (f32) -> d_points16 in `type` (kRowBF16 / kRowF16), freeing d_points.  fp16: refused (IDB_ERR_INVALID_ARG, the index
+    // unchanged) when a finite value would round to infinity; the message names the caller's row, input_row[PointId] when given.
+    idb_status narrow_points(uint32_t type, const uint32_t* input_row);
     // Storage for at least `rows` points: points, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
     // n rows.  Everything is allocated before anything is freed, so a failure leaves the index as it was.
     idb_status reserve_rows(uint64_t rows);
     // Rows [r0, r0 + m) (r0 >= n, within cap) from m x dim host floats, as the build stores them: zero padded, normalised for a
-    // cosine index, narrowed for a bf16 one; their zero rows INVALID; global_ids (m entries) into the id map when it exists.
+    // cosine index, narrowed for a bf16 / fp16 one; their zero rows INVALID; global_ids (m entries) into the id map when it exists.
+    // fp16 rows beyond its range are refused before anything of the index is written.
     idb_status stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids);
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
@@ -309,6 +314,14 @@ idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float
                      uint32_t n_ctrl);
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
+static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16, "RowType mirrors IDB_STORAGE_*");
+// fp16 storage: IDB_ERR_INVALID_ARG when an element of the m staged rows (nchunks * 4 f32 each, on the device) is finite and rounds to
+// +-infinity in fp16 (|x| >= 65520), naming the row (input_row[r] when given, else r + row0) and element; IDB_OK otherwise.
+idb_status check_f16_range(const float* d_rows, uint64_t m, uint32_t nchunks, const uint32_t* input_row, uint64_t row0, int num_sms,
+                           cudaStream_t st);
+// count elements f32 -> dst in `type` (kRowBF16 / kRowF16), round to nearest even; back to f32 exactly.  Enqueued on st.
+cudaError_t narrow_elems(const float* src, uint16_t* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st);
+cudaError_t widen_elems(const uint16_t* src, float* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st);
 // normalize_rows_kernel: dst[r] (nchunks * 4 floats, zero padded) = the canonical normalisation of src[r] (src_stride floats per row,
 // dim used, any alignment), one warp per row.  dst may equal src when src_stride == nchunks * 4.
 cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,
@@ -319,6 +332,11 @@ cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, ui
 idb_status merge_fits(const Index* ix, uint64_t lists, uint32_t k, int* max_smem);
 idb_status launch_merge(Index* ix, cudaStream_t st, const uint64_t* keys, uint32_t G, uint64_t nq, uint32_t k, uint32_t* d_ids,
                         float* d_dist, uint32_t* d_len, uint64_t* d_keys, int max_smem);
+
+// idb_index_from_graph_ex, and idb_index_load_storage with from_file (argument errors of the file's graph become IDB_ERR_FORMAT).
+idb_status adopt_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef_search, const uint32_t* zero,
+                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n, uint32_t storage, uint32_t metric,
+                       int32_t device, idb_index** out_index, bool from_file);
 
 cudaError_t ensure_u32(uint32_t*& p, size_t& cap, size_t need);
 cudaError_t ensure_u64(uint64_t*& p, size_t& cap, size_t need);

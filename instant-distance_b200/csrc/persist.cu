@@ -42,7 +42,7 @@ idb_status idb_index_save(const idb_index* index, const char* path) {
     std::vector<float> buf((size_t)chunk * ix->dim);
     for (uint64_t r0 = 0; ok && r0 < n; r0 += chunk) {
         const uint64_t m = std::min(chunk, n - r0);
-        idb_status st = ix->copy_points_f32(buf.data(), r0, m);  // bf16-stored rows are written widened (exact)
+        idb_status st = ix->copy_points_f32(buf.data(), r0, m);  // bf16- and fp16-stored rows are written widened (exact)
         if (st != IDB_OK) return st;
         ok = put(out.f, buf.data(), m * ix->dim * 4);
     }
@@ -73,10 +73,16 @@ idb_status idb_index_load(const char* path, uint32_t dim, uint32_t M, int32_t de
 
 idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M, uint32_t metric, int32_t device, idb_index** out_index,
                              uint64_t* out_values_offset) {
+    return idb_index_load_storage(path, dim, M, metric, IDB_STORAGE_F32, device, out_index, out_values_offset);
+}
+
+idb_status idb_index_load_storage(const char* path, uint32_t dim, uint32_t M, uint32_t metric, uint32_t storage, int32_t device,
+                                  idb_index** out_index, uint64_t* out_values_offset) {
     if (!path || !out_index) return fail(IDB_ERR_INVALID_ARG, "null argument");
     *out_index = nullptr;
     if (dim == 0 || M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "dim/M invalid");
     if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
+    if (storage > IDB_STORAGE_F16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
     File in;
     in.f = std::fopen(path, "rb");
     if (!in.f) return fail(IDB_ERR_IO, "cannot open %s", path);
@@ -107,10 +113,9 @@ idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M, uint32_
     for (uint32_t v : zero)
         if (v != IDB_INVALID && v >= n) return fail(IDB_ERR_FORMAT, "%s: adjacency refers to PointId %u >= %llu", path, v, (unsigned long long)n);
     // the same checks as for any adopted graph (entries inside their layer, n >= n_1 >= ... >= 1; for cosine, unit rows); a file that
-    // fails them is malformed
-    const idb_status st = idb_index_from_graph_ex(pts.data(), n, dim, M, (uint32_t)std::min<uint64_t>(ef, 0xFFFFFFFFu), zero.data(),
-                                                  (uint32_t)nl, ptrs.data(), counts.data(), IDB_STORAGE_F32, metric, device, out_index);
-    return st == IDB_ERR_INVALID_ARG ? IDB_ERR_FORMAT : st;
+    // fails them is malformed.  The rows were saved widened, so narrowing them again to the storage they came from is exact.
+    return adopt_graph(pts.data(), n, dim, M, (uint32_t)std::min<uint64_t>(ef, 0xFFFFFFFFu), zero.data(), (uint32_t)nl, ptrs.data(),
+                       counts.data(), storage, metric, device, out_index, true);
 }
 
 }  // extern "C"

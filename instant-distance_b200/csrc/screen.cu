@@ -19,8 +19,11 @@ namespace idb {
 
 namespace {
 
-__device__ __forceinline__ float stored_at(const void* pts, uint32_t bf16, size_t i) {
-    return bf16 ? __uint_as_float((uint32_t)reinterpret_cast<const uint16_t*>(pts)[i] << 16) : reinterpret_cast<const float*>(pts)[i];
+// Element i of the stored rows, widened exactly (row_type: RowType).
+__device__ __forceinline__ float stored_at(const void* pts, uint32_t row_type, size_t i) {
+    if (row_type == kRowF32) return reinterpret_cast<const float*>(pts)[i];
+    const uint32_t h = reinterpret_cast<const uint16_t*>(pts)[i];
+    return row_type == kRowBF16 ? __uint_as_float(h << 16) : widen_f16x2(h).x;
 }
 // order-preserving u32 image of a float (for atomicMin / atomicMax)
 __device__ __forceinline__ uint32_t ord_of(float f) {
@@ -30,7 +33,7 @@ __device__ __forceinline__ uint32_t ord_of(float f) {
 __device__ __forceinline__ float float_of_ord(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u); }
 
 // Blocks own ranges of rows, threads own elements: every step of a thread's loop is one coalesced slice of a row.
-__global__ void code_range_kernel(const void* pts, uint32_t bf16, uint64_t n, uint32_t stride, uint64_t rows_per_block, uint32_t* mn,
+__global__ void code_range_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint64_t rows_per_block, uint32_t* mn,
                                   uint32_t* mx, uint32_t* bad) {
     const uint64_t r0 = (uint64_t)blockIdx.x * rows_per_block, r1 = min(n, r0 + rows_per_block);
     if (r0 >= r1) return;
@@ -38,7 +41,7 @@ __global__ void code_range_kernel(const void* pts, uint32_t bf16, uint64_t n, ui
         float lo = INFINITY, hi = -INFINITY;
         bool nonfinite = false;
         for (uint64_t r = r0; r < r1; ++r) {
-            const float x = stored_at(pts, bf16, r * stride + e);
+            const float x = stored_at(pts, row_type, r * stride + e);
             nonfinite |= !isfinite(x);
             lo = fminf(lo, x);
             hi = fmaxf(hi, x);
@@ -66,7 +69,7 @@ __device__ __forceinline__ float code_of_value(float x, float offset, float step
     return step > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(x, offset), step)), 0.f), 255.f) : 0.f;
 }
 
-__global__ void code_encode_kernel(const void* pts, uint32_t bf16, uint64_t n, uint32_t stride, uint64_t rows_per_block, float* prm,
+__global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint64_t rows_per_block, float* prm,
                                    const uint32_t* step, unsigned char* codes) {
     const float S = __uint_as_float(*step);
     if (blockIdx.x == 0)
@@ -77,7 +80,7 @@ __global__ void code_encode_kernel(const void* pts, uint32_t bf16, uint64_t n, u
         const float offset = prm[stride + e];
         float err = 0.f;
         for (uint64_t r = r0; r < r1; ++r) {
-            const float x = stored_at(pts, bf16, r * stride + e);
+            const float x = stored_at(pts, row_type, r * stride + e);
             const float c = code_of_value(x, offset, S);
             codes[r * stride + e] = (unsigned char)c;
             const float xt = __fmaf_rn(c, S, offset);  // x~ of the per-element float bound
@@ -89,7 +92,7 @@ __global__ void code_encode_kernel(const void* pts, uint32_t bf16, uint64_t n, u
 
 // One warp per row (grid-stride): r_x = ||x - x~||, rounded up, with x~_i = offset_i + c_i * S in real arithmetic, which lies in
 // [fmaf_rd(c, S, offset), fmaf_ru(c, S, offset)], so |x_i - x~_i| <= max(x_i - lo, hi - x_i).  err_max = max over the rows.
-__global__ void code_row_err_kernel(const void* pts, uint32_t bf16, uint64_t n, uint32_t nchunks, const float* prm,
+__global__ void code_row_err_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t nchunks, const float* prm,
                                     const uint32_t* step, const uint32_t* codes, uint32_t* err_max) {
     const float S = __uint_as_float(*step);
     const uint32_t stride = nchunks * 4;
@@ -103,7 +106,7 @@ __global__ void code_row_err_kernel(const void* pts, uint32_t bf16, uint64_t n, 
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const uint32_t e = 4 * c + k;
-                const float x = stored_at(pts, bf16, r * stride + e), off = prm[stride + e], code = (float)((w >> (8 * k)) & 0xFFu);
+                const float x = stored_at(pts, row_type, r * stride + e), off = prm[stride + e], code = (float)((w >> (8 * k)) & 0xFFu);
                 const float d = fmaxf(__fsub_ru(x, __fmaf_rd(code, S, off)), __fsub_ru(__fmaf_ru(code, S, off), x));
                 acc = __fmaf_ru(d, d, acc);
             }
@@ -148,8 +151,7 @@ template <int CH>
 cudaError_t launch_screen_bound(const GraphView& g, const float4* q, const uint32_t* pairs, uint64_t npairs, float* ob, float* od,
                                 cudaStream_t st) {
     const unsigned grid = (unsigned)((npairs + 7) / 8);
-    if (g.bf16) screen_bound_kernel<CH, RowBF16><<<grid, 256, 0, st>>>(g, q, pairs, npairs, ob, od);
-    else screen_bound_kernel<CH, RowF32><<<grid, 256, 0, st>>>(g, q, pairs, npairs, ob, od);
+    with_row_type(g.row_type, [&](auto rt) { screen_bound_kernel<CH, decltype(rt)><<<grid, 256, 0, st>>>(g, q, pairs, npairs, ob, od); });
     return cudaGetLastError();
 }
 
@@ -162,7 +164,7 @@ idb_status Index::build_codes() {
     d_cparams = nullptr;
     if (!screen || n == 0) return IDB_OK;
     const uint32_t stride = nchunks * 4;
-    const void* pts = bf16 ? static_cast<const void*>(d_points_bf16) : static_cast<const void*>(d_points);
+    const void* pts = rows();
     const unsigned grid = (unsigned)std::min<uint64_t>((n + 63) / 64, (uint64_t)num_sms * 8);
     const uint64_t rows_per_block = (n + grid - 1) / grid;
     uint32_t* tmp = nullptr;  // [0, stride) min, [stride, 2 stride) max, [2 stride] non-finite flag, [2 stride + 1] S, [2 stride + 2] R
@@ -172,7 +174,7 @@ idb_status Index::build_codes() {
     if (e == cudaSuccess) e = fill_u32(tmp, stride, 0xFFFFFFFFu, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(tmp + stride, 0, ((size_t)stride + 3) * 4, stream);
     if (e == cudaSuccess) {
-        code_range_kernel<<<grid, 128, 0, stream>>>(pts, bf16 ? 1u : 0u, n, stride, rows_per_block, tmp, tmp + stride, tmp + 2 * stride);
+        code_range_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, rows_per_block, tmp, tmp + stride, tmp + 2 * stride);
         e = cudaGetLastError();
     }
     uint32_t bad = 0;
@@ -183,9 +185,9 @@ idb_status Index::build_codes() {
         float* prm = reinterpret_cast<float*>(d_cparams);
         uint32_t* step = tmp + 2 * stride + 1;
         code_params_kernel<<<(stride + 127) / 128, 128, 0, stream>>>(tmp, tmp + stride, stride, prm, step);
-        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, bf16 ? 1u : 0u, n, stride, rows_per_block, prm, step,
+        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, rows_per_block, prm, step,
                                                      reinterpret_cast<unsigned char*>(d_codes));
-        code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(pts, bf16 ? 1u : 0u, n, nchunks, prm, step, d_codes, step + 1);
+        code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(pts, row_type, n, nchunks, prm, step, d_codes, step + 1);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaMemcpyAsync(step_err, step, 8, cudaMemcpyDeviceToHost, stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream);

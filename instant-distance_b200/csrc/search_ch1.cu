@@ -3,8 +3,8 @@
 namespace idb {
 cudaError_t dispatch_search_ch1(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
     // tuning variants of the headline shape (ROW_T=2, EF_T=4): rows in flight per lane x resident CTAs per SM.  They are
-    // instantiated for f32 rows only: a bf16 index takes the default dispatch below.
-    if (a.variant && !a.g.bf16 && row_t <= 2 && ef_t <= 4) {
+    // instantiated for f32 rows only: a bf16 or fp16 index takes the default dispatch below.
+    if (a.variant && a.g.row_type == kRowF32 && row_t <= 2 && ef_t <= 4) {
         switch (a.variant) {
             case 1: return launch_search<1, 2, 4, 8, occ_for_warps(20)>(a, grid, st, win, 1);
             case 2: return launch_search<1, 2, 4, 8, occ_for_warps(24)>(a, grid, st, win, 2);

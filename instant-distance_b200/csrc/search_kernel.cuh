@@ -184,7 +184,7 @@ static cudaError_t launch_search(const SearchArgs& a, int grid, cudaStream_t str
     const int ring = TMA ? 64 + kSearchWarps * B * (int)a.g.nchunks * 16 : 0;
     cudaError_t e = launch_traversal<CH, EF_T>(search_kernel<CH, ROW_T, EF_T, B, OCC, RT, FULL, TMA>, a, ring, grid, stream, win);
     if (e == cudaSuccess && a.launched) {
-        const uint32_t cell[8] = {CH, ROW_T, EF_T, B, std::is_same<RT, RowBF16>::value ? 1u : 0u, FULL ? 1u : 0u, TMA ? 1u : 0u,
+        const uint32_t cell[8] = {CH, ROW_T, EF_T, B, RT::kType, FULL ? 1u : 0u, TMA ? 1u : 0u,
                                   (uint32_t)variant};
         std::memcpy(a.launched, cell, sizeof(cell));
     }
@@ -203,9 +203,12 @@ cudaError_t dispatch_row_ef_rt(const SearchArgs& a, int row_t, int ef_t, int gri
 }
 template <int CH, int B>
 cudaError_t dispatch_row_ef(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    // bf16 rows stay packed while in flight (half the registers per row): twice the rows in flight per lane
-    if (a.g.bf16) return dispatch_row_ef_rt<CH, (2 * B <= 16 ? 2 * B : B), RowBF16>(a, row_t, ef_t, grid, st, win);
-    return dispatch_row_ef_rt<CH, B, RowF32>(a, row_t, ef_t, grid, st, win);
+    // bf16 / fp16 rows stay packed while in flight (half the registers per row): twice the rows in flight per lane, up to 16
+    return with_row_type(a.g.row_type, [&](auto rt) {
+        using RT = decltype(rt);
+        constexpr int BR = RT::kChunkBytes == 8 && 2 * B <= 16 ? 2 * B : B;
+        return dispatch_row_ef_rt<CH, BR, RT>(a, row_t, ef_t, grid, st, win);
+    });
 }
 
 }  // namespace idb

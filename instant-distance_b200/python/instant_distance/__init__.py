@@ -11,7 +11,10 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
   * `Hnsw.insert / HnswMap.insert` append points to a built or loaded index (layer 0 only, PointIds continue from the current
     count; DESIGN.md §6);
   * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
-    DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it.
+    DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it;
+  * `Config.storage = "bf16"` or `"f16"` keeps the points in GPU memory rounded to 2 bytes per element (default "f32"; DESIGN.md
+    §3b: results are those of the f32 index on the rounded points; "f16" refuses values that round to infinity, |x| >= 65520).
+    The file holds the points widened to f32, so `Hnsw.load / HnswMap.load(..., storage=)` take the storage too.
 """
 import ctypes as C
 import random
@@ -42,9 +45,11 @@ class Config:
         self.seed = random.getrandbits(64)
         self.heuristic = Heuristic()
         self.metric = "l2sq"  # or "cosine"
+        self.storage = "f32"  # or "bf16", "f16"
 
     def _params(self):
-        kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed, metric=self.metric)
+        kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed, metric=self.metric,
+                  storage=_abi._storage(self.storage))
         if self.heuristic is None:
             kw["heuristic"] = 0
         else:
@@ -159,10 +164,10 @@ class Hnsw:
         self._ix.save(fname)
 
     @staticmethod
-    def load(fname, dim=300, M=32, metric="l2sq"):
-        """py:121-129.  The file does not store dim / M (fixed arrays in the reference: 300 / 32), nor the metric."""
+    def load(fname, dim=300, M=32, metric="l2sq", storage="f32"):
+        """py:121-129.  The file does not store dim / M (fixed arrays in the reference: 300 / 32), nor the metric or storage."""
         try:
-            ix, _ = _abi.Index.load(fname, dim, M, metric=metric)
+            ix, _ = _abi.Index.load(fname, dim, M, metric=metric, storage=storage)
         except _abi.IdbError as e:
             if e.status == _abi.ERR_IO:
                 raise OSError(str(e)) from e
@@ -210,12 +215,12 @@ class HnswMap(Hnsw):
                 f.write(struct.pack("<IQ", 0, len(b)) + b)
 
     @staticmethod
-    def load(fname, dim=300, M=32, metric="l2sq"):
+    def load(fname, dim=300, M=32, metric="l2sq", storage="f32"):
         """py:58-67."""
         import struct
 
         try:
-            ix, off = _abi.Index.load(fname, dim, M, metric=metric)
+            ix, off = _abi.Index.load(fname, dim, M, metric=metric, storage=storage)
         except _abi.IdbError as e:
             if e.status == _abi.ERR_IO:
                 raise OSError(str(e)) from e

@@ -25,7 +25,7 @@ SYMBOLS = [
     "idb_sharded_search_batch_device", "idb_sharded_search_batch_f32_multi", "idb_sharded_search_batch_device_multi", "idb_distance_f32", "idb_host_alloc", "idb_host_free", "idb_last_error", "idb_version", "idb_device_count",
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
-    "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32",
+    "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32", "idb_index_load_storage",
 ]
 
 
@@ -73,6 +73,7 @@ def lib():
     L.idb_index_from_graph_ex.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_uint32,
                                           C.POINTER(u32p), u64p, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp)]
     L.idb_index_load_ex.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
+    L.idb_index_load_storage.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
     L.idb_index_insert_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), u32p, u32p]
     L.idb_normalize_f32.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_int32, f32p]
     L.idb_index_metric.argtypes = [vp, u32p]
@@ -145,7 +146,7 @@ def ptr(a, t):
     return a.ctypes.data_as(C.POINTER(t))
 
 
-STORAGE = {"f32": 0, "bf16": 1}
+STORAGE = {"f32": 0, "bf16": 1, "f16": 2}  # IDB_STORAGE_*: how an index keeps its rows (2-byte rows are widened exactly to f32)
 METRIC = {"l2sq": 0, "cosine": 1}  # IDB_METRIC_*: squared L2, or 1 - cos through canonically normalised rows (DESIGN.md §3a)
 
 
@@ -153,6 +154,12 @@ def _metric(metric):
     if metric not in METRIC:
         raise ValueError(f"metric must be one of {sorted(METRIC)}, not {metric!r}")
     return METRIC[metric]
+
+
+def _storage(storage):
+    if storage not in STORAGE:
+        raise ValueError(f"storage must be one of {sorted(STORAGE)}, not {storage!r}")
+    return STORAGE[storage]
 PROGRESS_FN = C.CFUNCTYPE(None, C.c_uint64, C.c_uint64, C.c_void_p)
 
 
@@ -241,10 +248,12 @@ class Index:
         check(lib().idb_index_save(self._h, os.fsencode(path)))
 
     @classmethod
-    def load(cls, path, dim=300, M=32, device=0, metric="l2sq"):
-        """Returns (Index, offset of the HnswMap values in the file).  The file does not record the metric."""
+    def load(cls, path, dim=300, M=32, device=0, metric="l2sq", storage="f32"):
+        """Returns (Index, offset of the HnswMap values in the file).  The file records neither the metric nor the storage: it
+        holds f32 rows, stored again as `storage` ("f32", "bf16" or "f16")."""
         h, off = C.c_void_p(), C.c_uint64()
-        check(lib().idb_index_load_ex(os.fsencode(path), dim, M, _metric(metric), device, C.byref(h), C.byref(off)))
+        check(lib().idb_index_load_storage(os.fsencode(path), dim, M, _metric(metric), _storage(storage), device, C.byref(h),
+                                           C.byref(off)))
         return cls(h), int(off.value)
 
     def info(self):
@@ -318,7 +327,8 @@ class Index:
     KERNEL_FIELDS = ("ch", "row_t", "ef_t", "b", "bf16", "full", "tma", "variant")
 
     def last_kernel(self, lane=0xFFFFFFFF):
-        """The search-kernel instantiation the last call launched, as a dict over KERNEL_FIELDS (all zeros: none launched)."""
+        """The search-kernel instantiation the last call launched, as a dict over KERNEL_FIELDS (all zeros: none launched).
+        The "bf16" field carries the row type, a STORAGE value: 0 f32, 1 bf16, 2 f16."""
         out = (C.c_uint32 * 8)()
         check(lib().idb_last_search_kernel(self._h, lane, out))
         return dict(zip(self.KERNEL_FIELDS, (int(v) for v in out)))

@@ -33,6 +33,8 @@ extern "C" {
                                upper: *const *const u32, upper_n: *const u64, storage: u32, metric: u32, device: i32,
                                out: *mut *mut IdbIndex) -> i32;
     fn idb_index_load_ex(path: *const c_char, dim: u32, m: u32, metric: u32, device: i32, out: *mut *mut IdbIndex, values_offset: *mut u64) -> i32;
+    fn idb_index_load_storage(path: *const c_char, dim: u32, m: u32, metric: u32, storage: u32, device: i32, out: *mut *mut IdbIndex,
+                              values_offset: *mut u64) -> i32;
     fn idb_normalize_f32(rows: *const f32, n: u64, dim: u32, device: i32, out: *mut f32) -> i32;
     fn idb_index_metric(ix: *const IdbIndex, out: *mut u32) -> i32;
     fn idb_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, ef: u32, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
@@ -73,6 +75,12 @@ impl Point for F32Point {
 /// points and queries (DESIGN.md §3a).  `F32Point::distance` stays squared L2.
 pub const METRIC_L2SQ: u32 = 0;
 pub const METRIC_COSINE: u32 = 1;
+
+/// How an index stores its rows (include/instant_distance_b200.h IDB_STORAGE_*, the `storage` field of `IdbParams`): f32, or rounded
+/// to bf16 / fp16 (half the bytes; fp16 refuses values that round to infinity).  Distances stay fp32 on the exactly widened rows.
+pub const STORAGE_F32: u32 = 0;
+pub const STORAGE_BF16: u32 = 1;
+pub const STORAGE_F16: u32 = 2;
 
 /// The canonical normalisation the cosine metric applies, evaluated on `device` (rows: n x dim, row-major).
 pub fn normalize(rows: &[f32], dim: usize, device: i32) -> Vec<f32> {
