@@ -361,7 +361,7 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
         cudaFree(d_rows);
         cudaFree(d_order);
     }
-    if (p.storage != IDB_STORAGE_F32) {  // fp16: rows beyond its range are refused here, named by their input row
+    if (p.storage != IDB_STORAGE_F32) {  // fp16 / q8: rows beyond the storage's range are refused here, named by their input row
         idb_status sb = ix->narrow_points(p.storage, order.data());
         if (sb != IDB_OK) return sb;
     }
@@ -413,8 +413,8 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
 // Construction::insert(new, 0, layers) (core:437-528) for PointIds [n0, n0 + m), in the build's layer-0 batch schedule from g0 = n0
 // (also when the index has no upper layer, where the build inserts sequentially).  The caller holds the index exclusively and has
 // checked the arguments.  Rows: m x dim host floats, stored as the build stores them (zero padded, normalised for a cosine index,
-// then narrowed for a bf16 or fp16 one; fp16 rows beyond its range are refused before the index's rows or graph change).  global_ids:
-// appended to the id map when the index has one.
+// then narrowed for a bf16 or fp16 one or quantised for a q8 one; fp16 / q8 rows beyond the storage's range are refused before
+// the index's rows or graph change).  global_ids: appended to the id map when the index has one.
 idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_params& p, const uint32_t* global_ids, uint32_t* out_ids) {
     const uint64_t n0 = ix->n, n1 = n0 + m;
     if (out_ids)
@@ -477,7 +477,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
         return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", params->ef_construction);
     if (dim > 10240) return fail(IDB_ERR_UNSUPPORTED, "dim %u > 10240 is not supported (the owner row of a long-row traversal lives in shared memory)", dim);
     if (!(params->ml > 0.0f) || params->ml >= 1.0f) return fail(IDB_ERR_INVALID_ARG, "ml must be in (0, 1)");
-    if (params->storage > IDB_STORAGE_F16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
+    if (!storage_known(params->storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
     if (params->heuristic && params->extend_candidates)
         return fail(IDB_ERR_UNSUPPORTED,
                     "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "

@@ -65,7 +65,7 @@ __device__ __forceinline__ uint32_t select_heuristic_warp(const GraphView& g, co
     bool cok[CH > 0 ? CH : 1];
 #pragma unroll
     for (int j = 0; j < (CH > 0 ? CH : 1); ++j) cok[j] = (uint32_t)(lane + 32 * j) < g.nchunks;
-    const uint32_t row_bytes = g.nchunks * RT::kChunkBytes;   // global rows (f32, bf16 or fp16)
+    const uint32_t row_bytes = g.nchunks * RT::kChunkBytes;   // global rows (f32, bf16, fp16 or q8)
     const uint32_t srow_bytes = g.nchunks * 16u;               // staged rows are always widened float4
     const char* gbase = g.points + lane * RT::kChunkBytes;
     const char* sbase = reinterpret_cast<const char*>(kept_vecs) + lane * 16;
@@ -91,11 +91,14 @@ __device__ __forceinline__ uint32_t select_heuristic_warp(const GraphView& g, co
 #pragma unroll
             for (int r = 0; r < NB; ++r) {
                 const bool ok = (uint32_t)r < nb;  // branch-free: predicated loads, see batch_distances
-                const char* row = kStage ? sbase + (size_t)(b0 + r) * srow_bytes
-                                         : gbase + (size_t)(ok ? kept_pid[b0 + r] : 0u) * row_bytes;
+                const uint32_t rp = ok ? kept_pid[b0 + r] : 0u;
+                const char* row = kStage ? sbase + (size_t)(b0 + r) * srow_bytes : gbase + (size_t)rp * row_bytes;
+                typename RT::Hdr h = typename RT::Hdr();
+                if (!kStage) h = RT::hdr(g, rp);
 #pragma unroll
                 for (int j = 0; j < CH; ++j)
-                    v[r][j] = (ok && cok[j]) ? (kStage ? *reinterpret_cast<const float4*>(row + j * 512) : RT::ld(row + j * 32 * RT::kChunkBytes))
+                    v[r][j] = (ok && cok[j]) ? (kStage ? *reinterpret_cast<const float4*>(row + j * 512)
+                                                       : widen_chunk<RT>(g, RT::ld_raw(row + j * 32 * RT::kChunkBytes), h, lane + 32 * j))
                                              : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             float p[NB];

@@ -113,10 +113,12 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
         float d[QW];
         if constexpr (CH == 0) {  // batch_distances_long's order: four chains per row carried across groups of 32 chunks
             const char* row[NB];
+            typename RT::Hdr h[NB];
             float4 acc[NB];
 #pragma unroll
             for (int i = 0; i < NB; ++i) {
                 row[i] = lane_base + (size_t)(b0 + ((uint32_t)i < nb ? i : 0)) * row_bytes;
+                h[i] = RT::hdr(a.g, (uint32_t)(b0 + ((uint32_t)i < nb ? i : 0)));
                 acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
 #pragma unroll 1
@@ -127,7 +129,7 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
 #pragma unroll
                 for (int i = 0; i < NB; ++i) v[i] = (ok && (uint32_t)i < nb) ? RT::ld_raw(row[i] + (size_t)j * 32 * RT::kChunkBytes) : RT::zero();
 #pragma unroll
-                for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, RT::widen(v[i]));
+                for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, widen_chunk<RT>(a.g, v[i], h[i], lane + 32u * j));
             }
             float p[NB];
 #pragma unroll
@@ -135,10 +137,12 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
             d[0] = batch_butterfly<NB>(p, lane);
         } else {  // batch_distances_impl's order, the rows shared by the warp's QW queries
             typename RT::Raw v[NB][CH];
+            typename RT::Hdr h[NB];
 #pragma unroll
             for (int i = 0; i < NB; ++i) {
                 const bool ok = (uint32_t)i < nb;
                 const char* row = lane_base + (size_t)(b0 + (ok ? i : 0)) * row_bytes;
+                h[i] = RT::hdr(a.g, (uint32_t)(b0 + (ok ? i : 0)));
 #pragma unroll
                 for (int j = 0; j < CH; ++j)
                     v[i][j] = (ok && (uint32_t)(lane + 32 * j) < nchunks) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
@@ -147,7 +151,7 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
             for (int qj = 0; qj < QW; ++qj) {
                 float p[NB];
 #pragma unroll
-                for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(q[qj].r, v[i]);
+                for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(a.g, q[qj].r, v[i], h[i], lane);
                 d[qj] = batch_butterfly<NB>(p, lane);  // lane l: row b0 + (l & (NB - 1))
             }
         }

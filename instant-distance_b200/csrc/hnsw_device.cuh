@@ -35,12 +35,13 @@ constexpr uint32_t kFullMask = 0xFFFFFFFFu;
 enum OptFlags : uint32_t { kOptPrefetchVectors = 1u, kOptPrefetchRows = 2u, kOptPrefetchNextRow = 8u };
 
 // How an index stores its rows; the values are the ABI's IDB_STORAGE_* (internal.cuh checks that).
-enum RowType : uint32_t { kRowF32 = 0, kRowBF16 = 1, kRowF16 = 2 };
+enum RowType : uint32_t { kRowF32 = 0, kRowBF16 = 1, kRowF16 = 2, kRowQ8 = 4 };
 
 enum QueryStatus : uint32_t { kQueryOk = 0, kQueryVisitedOverflow = 1, kQueryTieOverflow = 2 };
 
 struct GraphView {
-    const char* points;          // n rows of nchunks 4-element chunks (dim rounded up to 4, zero padded); f32 (16 B/chunk), bf16 or fp16 (8 B/chunk)
+    const char* points;          // n rows of nchunks 4-element chunks (dim rounded up to 4, zero padded); f32 (16 B/chunk), bf16 or fp16
+                                 // (8 B/chunk), q8 (4 B/chunk: one code byte per element)
     uint32_t nchunks;            // 4-element chunks per row
     const uint32_t* zero;        // n x 2M
     const uint32_t* const* upper;  // device array: upper[l-1] = n_l x M
@@ -54,6 +55,10 @@ struct GraphView {
     const float4* cparams;       // 3 x nchunks float4: per element scale, offset, E (x~ = fmaf(code, scale, offset), |x - x~| <= E)
     float cstep;                 // S: the one code step of every element (the scale slots of cparams all hold it)
     float cerr;                  // R >= ||x - x~|| over every stored row, x~_i = offset_i + code_i * S in real arithmetic
+    // q8 rows (DESIGN §3c), else unused: row r's header {o, s} (element i = fmaf(code_i, s, o)), and how many elements of the last
+    // chunk belong to the row (1..4; the codes of the padding do not widen to zero, so the loaders zero them)
+    const float2* hdr;
+    uint32_t tail;
 };
 
 // ---------------------------------------------------------------------------------------------------------
@@ -81,29 +86,36 @@ __device__ __forceinline__ float lane_partial(const float4 (&q)[CH], const float
 
 // Row storage types.  A lane always owns the same 4 ELEMENTS per 128-element block (chunk l, l+32, ...), so the canonical
 // fp32 summation order is the same for all of them; bf16 and fp16 rows are widened exactly (bf16 -> f32 is a 16-bit shift, fp16 -> f32
-// is cvt.f32.f16, exact for every fp16 value, subnormals included).
-// `Raw` is what a lane keeps in registers while a batch of row loads is in flight (bf16 / fp16 rows stay packed: half the
-// registers per row, so twice as many rows in flight); widen() runs at the point of use.
+// is cvt.f32.f16, exact for every fp16 value, subnormals included), and so are q8 rows (DESIGN §3c: (b + c) 2^e is an f32, so
+// fmaf(c, 2^e, b 2^e) is exact however it is evaluated).
+// `Raw` is what a lane keeps in registers while a batch of row loads is in flight (bf16 / fp16 / q8 rows stay packed: a half or a
+// quarter of the registers per row, so more rows in flight); widen() runs at the point of use.  `Hdr` is what a row carries besides its
+// chunks, fetched once per row with hdr(): empty except for q8, whose rows have a grid of their own.
+struct NoHdr {};
 struct RowF32 {
     static constexpr uint32_t kType = kRowF32;
     static constexpr uint32_t kChunkBytes = 16;
     using Raw = float4;
+    using Hdr = NoHdr;
+    static __device__ __forceinline__ Hdr hdr(const GraphView&, uint32_t) { return Hdr(); }
     static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
     static __device__ __forceinline__ Raw zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-    static __device__ __forceinline__ float4 widen(Raw r) { return r; }
-    static __device__ __forceinline__ float4 ld(const char* p) { return ld_raw(p); }
+    static __device__ __forceinline__ float4 widen(Raw r, Hdr) { return r; }
+    static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
 };
 struct RowBF16 {
     static constexpr uint32_t kType = kRowBF16;
     static constexpr uint32_t kChunkBytes = 8;
     using Raw = uint2;
+    using Hdr = NoHdr;
+    static __device__ __forceinline__ Hdr hdr(const GraphView&, uint32_t) { return Hdr(); }
     static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
     static __device__ __forceinline__ Raw zero() { return make_uint2(0u, 0u); }
-    static __device__ __forceinline__ float4 widen(Raw u) {
+    static __device__ __forceinline__ float4 widen(Raw u, Hdr) {
         return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
                            __uint_as_float(u.y & 0xFFFF0000u));
     }
-    static __device__ __forceinline__ float4 ld(const char* p) { return widen(ld_raw(p)); }
+    static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
 };
 // The two fp16 values packed in u (element 2i in the low half), widened exactly.
 __device__ __forceinline__ float2 widen_f16x2(uint32_t u) {
@@ -117,35 +129,74 @@ struct RowF16 {
     static constexpr uint32_t kType = kRowF16;
     static constexpr uint32_t kChunkBytes = 8;
     using Raw = uint2;
+    using Hdr = NoHdr;
+    static __device__ __forceinline__ Hdr hdr(const GraphView&, uint32_t) { return Hdr(); }
     static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
     static __device__ __forceinline__ Raw zero() { return make_uint2(0u, 0u); }
-    static __device__ __forceinline__ float4 widen(Raw u) {
+    static __device__ __forceinline__ float4 widen(Raw u, Hdr) {
         const float2 a = widen_f16x2(u.x), b = widen_f16x2(u.y);
         return make_float4(a.x, a.y, b.x, b.y);
     }
-    static __device__ __forceinline__ float4 ld(const char* p) { return widen(ld_raw(p)); }
+    static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
+};
+// q8 (DESIGN §3c): one code byte per element (byte k of a chunk's word = element 4c+k, the screening codes' layout) and a per-row
+// header {o, s} = {b 2^e, 2^e}; element i = fmaf(c_i, s, o), exact.  A zero Hdr widens every code to 0 (rows past the batch).
+struct RowQ8 {
+    static constexpr uint32_t kType = kRowQ8;
+    static constexpr uint32_t kChunkBytes = 4;
+    using Raw = uint32_t;
+    using Hdr = float2;
+    static __device__ __forceinline__ Hdr hdr(const GraphView& g, uint32_t pid) { return __ldg(g.hdr + pid); }
+    static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const uint32_t*>(p)); }
+    static __device__ __forceinline__ Raw zero() { return 0u; }
+    static __device__ __forceinline__ float4 widen(Raw u, Hdr h) {
+        return make_float4(__fmaf_rn((float)(u & 0xFFu), h.y, h.x), __fmaf_rn((float)((u >> 8) & 0xFFu), h.y, h.x),
+                           __fmaf_rn((float)((u >> 16) & 0xFFu), h.y, h.x), __fmaf_rn((float)(u >> 24), h.y, h.x));
+    }
+    static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
 };
 // f(RT()) for the row type `row_type` of an index: the one place a run-time row type becomes a template argument.
 template <class F>
 auto with_row_type(uint32_t row_type, F&& f) {
     if (row_type == kRowBF16) return f(RowBF16());
     if (row_type == kRowF16) return f(RowF16());
+    if (row_type == kRowQ8) return f(RowQ8());
     return f(RowF32());
+}
+// Chunk c of a row, widened.  The zero padding of f32 / bf16 / fp16 rows, and the zero Raw loaders put in place of chunks past the
+// row, widen to zeros.  q8 codes widen to o instead, so for q8 the elements past the row (in its last chunk, and every chunk c >=
+// nchunks) are zeroed here.  (FULL cells too: every chunk is real there, but the last one may still end past dim.)
+template <class RT>
+__device__ __forceinline__ float4 widen_chunk(const GraphView& g, typename RT::Raw r, typename RT::Hdr h, uint32_t c) {
+    float4 v = RT::widen(r, h);
+    if constexpr (RT::kType == kRowQ8) {
+        if (c + 1u >= g.nchunks) {
+            const uint32_t t = c + 1u == g.nchunks ? g.tail : 0u;
+            if (t < 1u) v.x = 0.f;
+            if (t < 2u) v.y = 0.f;
+            if (t < 3u) v.z = 0.f;
+            if (t < 4u) v.w = 0.f;
+        }
+    }
+    return v;
 }
 // This lane's CH chunks of row `pid` (zeros beyond the row's last chunk).
 template <int CH, class RT>
 __device__ __forceinline__ void load_row(const GraphView& g, uint32_t pid, int lane, float4 (&q)[CH]) {
     const char* row = g.points + (size_t)pid * (g.nchunks * RT::kChunkBytes) + lane * RT::kChunkBytes;
+    const typename RT::Hdr h = RT::hdr(g, pid);
 #pragma unroll
     for (int j = 0; j < CH; ++j)
-        q[j] = (uint32_t)(lane + 32 * j) < g.nchunks ? RT::ld(row + j * 32 * RT::kChunkBytes) : make_float4(0.f, 0.f, 0.f, 0.f);
+        q[j] = (uint32_t)(lane + 32 * j) < g.nchunks ? widen_chunk<RT>(g, RT::ld_raw(row + j * 32 * RT::kChunkBytes), h, lane + 32 * j)
+                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 template <int CH, class RT>
-__device__ __forceinline__ float lane_partial_raw(const float4 (&q)[CH], const typename RT::Raw (&r)[CH]) {
+__device__ __forceinline__ float lane_partial_raw(const GraphView& g, const float4 (&q)[CH], const typename RT::Raw (&r)[CH],
+                                                  typename RT::Hdr h, int lane) {
     float4 v[CH];
 #pragma unroll
-    for (int j = 0; j < CH; ++j) v[j] = RT::widen(r[j]);
+    for (int j = 0; j < CH; ++j) v[j] = widen_chunk<RT>(g, r[j], h, lane + 32 * j);
     return lane_partial<CH>(q, v);
 }
 
@@ -182,9 +233,10 @@ template <int CH, class RT>
 __device__ __forceinline__ void q_from_point(QVec<CH>& q, const GraphView& g, uint32_t pid, int lane) {
     if constexpr (CH == 0) {
         const char* row = g.points + (size_t)pid * (g.nchunks * RT::kChunkBytes);
+        const typename RT::Hdr h = RT::hdr(g, pid);
         __syncwarp();  // earlier readers of the buffer are done
         for (uint32_t c = lane; c < q.ngroups * 32u; c += 32)
-            q.s[c] = c < g.nchunks ? RT::ld(row + (size_t)c * RT::kChunkBytes) : make_float4(0.f, 0.f, 0.f, 0.f);
+            q.s[c] = c < g.nchunks ? widen_chunk<RT>(g, RT::ld_raw(row + (size_t)c * RT::kChunkBytes), h, c) : make_float4(0.f, 0.f, 0.f, 0.f);
         __syncwarp();
     } else {
         load_row<CH, RT>(g, pid, lane, q.r);
@@ -704,10 +756,12 @@ __device__ __forceinline__ void batch_distances_impl(const GraphView& g, const f
     for (uint32_t b0 = 0; b0 < n_new; b0 += NB) {
         const uint32_t nb = n_new - b0;  // rows in this batch (uniform); entries i >= nb are predicated off
         typename RT::Raw v[NB][CH];
+        typename RT::Hdr h[NB];
         if (kFull && nb >= (uint32_t)NB) {  // uniform; two of the ~three trips per expansion: plain loads, no predicates, no zero fill
 #pragma unroll
             for (int i = 0; i < NB; ++i) {
                 const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
+                h[i] = RT::hdr(g, cpid[b0 + i]);
 #pragma unroll
                 for (int j = 0; j < CH; ++j) v[i][j] = RT::ld_raw(row + j * 32 * RT::kChunkBytes);
             }
@@ -717,6 +771,7 @@ __device__ __forceinline__ void batch_distances_impl(const GraphView& g, const f
                 // branch-free on purpose: `if (i < nb) {load; use}` makes ptxas emit two branches per row
                 const bool ok = (uint32_t)i < nb;
                 const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
+                h[i] = ok ? RT::hdr(g, cpid[b0 + i]) : typename RT::Hdr();
 #pragma unroll
                 for (int j = 0; j < CH; ++j)
                     v[i][j] = (ok && cok[j]) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
@@ -724,7 +779,7 @@ __device__ __forceinline__ void batch_distances_impl(const GraphView& g, const f
         }
         float p[NB];
 #pragma unroll
-        for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(q, v[i]);
+        for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(g, q, v[i], h[i], lane);
         const float total = batch_butterfly<NB>(p, lane);
         if ((uint32_t)lane < nb && lane < NB) ckey[b0 + lane] = mk_key(total, cpid[b0 + lane]);
     }
@@ -740,10 +795,12 @@ __device__ __forceinline__ void batch_distances_long(const GraphView& g, const Q
     for (uint32_t b0 = 0; b0 < n_new; b0 += NB) {
         const uint32_t nb = n_new - b0;
         const char* row[NB];
+        typename RT::Hdr h[NB];
         float4 acc[NB];
 #pragma unroll
         for (int i = 0; i < NB; ++i) {
             row[i] = lane_base + (size_t)cpid[b0 + ((uint32_t)i < nb ? i : 0)] * row_bytes;
+            h[i] = RT::hdr(g, cpid[b0 + ((uint32_t)i < nb ? i : 0)]);
             acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll 1
@@ -754,7 +811,7 @@ __device__ __forceinline__ void batch_distances_long(const GraphView& g, const Q
 #pragma unroll
             for (int i = 0; i < NB; ++i) v[i] = (ok && (uint32_t)i < nb) ? RT::ld_raw(row[i] + (size_t)j * 32 * RT::kChunkBytes) : RT::zero();
 #pragma unroll
-            for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, RT::widen(v[i]));
+            for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, widen_chunk<RT>(g, v[i], h[i], lane + 32u * j));
         }
         float p[NB];
 #pragma unroll
@@ -1034,7 +1091,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
 #ifdef IDB_K1_PHASES
     k1_phase_begin(s);
 #endif
-    constexpr bool kScreen = SCREEN && CH > 0 && !kLive && !TMA;
+    constexpr bool kScreen = SCREEN && CH > 0 && !kLive && !TMA && RT::kType != kRowQ8;  // (q8: no table, DESIGN §3c)
     ScreenQuery<kScreen ? CH : 1> sq;
     if constexpr (kScreen) {
         if (g.codes) screen_query<CH>(sq, g, q.r, lane);

@@ -207,8 +207,10 @@ struct Index {
     std::atomic<uint64_t> n{0};                // written by an insert while other threads may read it (searches take a lane first)
     uint64_t cap = 0;                          // rows allocated for points, zero and the id map (>= n; grows by doubling on insert)
     uint32_t dim = 0, nchunks = 0, M = 32, ef_search = 100;
-    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored in 2 bytes
+    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored narrower
     uint16_t* d_points16 = nullptr;            // cap x nchunks*4 bf16 or fp16 (row_type kRowBF16 / kRowF16), else null
+    uint8_t* d_points8 = nullptr;              // cap x nchunks*4 q8 codes (row_type kRowQ8), else null
+    float2* d_hdr = nullptr;                   // cap q8 row headers {o, s} (DESIGN §3c), else null
     uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
     uint32_t* d_zero = nullptr;                // cap x 2M (rows past n: INVALID)
@@ -249,17 +251,21 @@ struct Index {
     idb_status upload(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef, const uint32_t* zero,
                       uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
-    uint32_t elem_bytes() const { return row_type == kRowF32 ? 4u : 2u; }
-    const void* rows() const { return row_type == kRowF32 ? static_cast<const void*>(d_points) : static_cast<const void*>(d_points16); }
-    // d_points (f32) -> d_points16 in `type` (kRowBF16 / kRowF16), freeing d_points.  fp16: refused (IDB_ERR_INVALID_ARG, the index
-    // unchanged) when a finite value would round to infinity; the message names the caller's row, input_row[PointId] when given.
+    uint32_t elem_bytes() const { return row_type == kRowF32 ? 4u : row_type == kRowQ8 ? 1u : 2u; }
+    const void* rows() const {
+        return row_type == kRowF32 ? static_cast<const void*>(d_points)
+               : row_type == kRowQ8 ? static_cast<const void*>(d_points8) : static_cast<const void*>(d_points16);
+    }
+    // d_points (f32) -> d_points16 in `type` (kRowBF16 / kRowF16), or d_points8 + d_hdr (kRowQ8), freeing d_points.  fp16 / q8:
+    // refused (IDB_ERR_INVALID_ARG, the index unchanged) when a row is beyond the storage's range (check_f16_range, check_q8_rows);
+    // the message names the caller's row, input_row[PointId] when given.
     idb_status narrow_points(uint32_t type, const uint32_t* input_row);
     // Storage for at least `rows` points: points, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
     // n rows.  Everything is allocated before anything is freed, so a failure leaves the index as it was.
     idb_status reserve_rows(uint64_t rows);
     // Rows [r0, r0 + m) (r0 >= n, within cap) from m x dim host floats, as the build stores them: zero padded, normalised for a
-    // cosine index, narrowed for a bf16 / fp16 one; their zero rows INVALID; global_ids (m entries) into the id map when it exists.
-    // fp16 rows beyond its range are refused before anything of the index is written.
+    // cosine index, narrowed for a bf16 / fp16 one, quantised for a q8 one; their zero rows INVALID; global_ids (m entries) into the
+    // id map when it exists.  fp16 / q8 rows beyond the storage's range are refused before anything of the index is written.
     idb_status stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids);
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
@@ -314,7 +320,18 @@ idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float
                      uint32_t n_ctrl);
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
-static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16, "RowType mirrors IDB_STORAGE_*");
+static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16 && kRowQ8 == IDB_STORAGE_Q8,
+              "RowType mirrors IDB_STORAGE_*");
+// The storage values an index accepts (3 is not one of them).
+inline bool storage_known(uint32_t s) { return s <= IDB_STORAGE_F16 || s == IDB_STORAGE_Q8; }
+// q8 storage (DESIGN §3c): IDB_ERR_INVALID_ARG when one of the m staged rows (nchunks * 4 f32 each, the first dim used, on the device)
+// has a NaN or infinite element, or its header or a dequantised element would overflow f32; the message names the row (input_row[r]
+// when given, else r + row0) and element.  IDB_OK otherwise.
+idb_status check_q8_rows(const float* d_rows, uint64_t m, uint32_t nchunks, uint32_t dim, const uint32_t* input_row, uint64_t row0,
+                         int num_sms, cudaStream_t st);
+// m checked rows (nchunks * 4 f32 each) -> their codes (nchunks * 4 bytes each, padding codes 0) and headers.  Enqueued on st.
+cudaError_t quantize_q8(const float* src, uint64_t m, uint32_t nchunks, uint32_t dim, uint8_t* codes, float2* hdr, int num_sms,
+                        cudaStream_t st);
 // fp16 storage: IDB_ERR_INVALID_ARG when an element of the m staged rows (nchunks * 4 f32 each, on the device) is finite and rounds to
 // +-infinity in fp16 (|x| >= 65520), naming the row (input_row[r] when given, else r + row0) and element; IDB_OK otherwise.
 idb_status check_f16_range(const float* d_rows, uint64_t m, uint32_t nchunks, const uint32_t* input_row, uint64_t row0, int num_sms,

@@ -82,7 +82,7 @@ idb_status idb_index_load_storage(const char* path, uint32_t dim, uint32_t M, ui
     *out_index = nullptr;
     if (dim == 0 || M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "dim/M invalid");
     if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
-    if (storage > IDB_STORAGE_F16) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
+    if (!storage_known(storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
     File in;
     in.f = std::fopen(path, "rb");
     if (!in.f) return fail(IDB_ERR_IO, "cannot open %s", path);

@@ -203,10 +203,11 @@ cudaError_t dispatch_row_ef_rt(const SearchArgs& a, int row_t, int ef_t, int gri
 }
 template <int CH, int B>
 cudaError_t dispatch_row_ef(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    // bf16 / fp16 rows stay packed while in flight (half the registers per row): twice the rows in flight per lane, up to 16
+    // bf16 / fp16 / q8 rows stay packed while in flight (a half or a quarter of the registers per row): twice the rows in flight per
+    // lane, up to 16 (q8 takes the 2-byte rule: it also carries a header per row)
     return with_row_type(a.g.row_type, [&](auto rt) {
         using RT = decltype(rt);
-        constexpr int BR = RT::kChunkBytes == 8 && 2 * B <= 16 ? 2 * B : B;
+        constexpr int BR = RT::kChunkBytes <= 8 && 2 * B <= 16 ? 2 * B : B;
         return dispatch_row_ef_rt<CH, BR, RT>(a, row_t, ef_t, grid, st, win);
     });
 }

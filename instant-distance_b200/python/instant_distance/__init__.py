@@ -14,6 +14,8 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
     DESIGN.md §3a; default "l2sq"); the file does not record it, so `Hnsw.load / HnswMap.load(..., metric=)` take it;
   * `Config.storage = "bf16"` or `"f16"` keeps the points in GPU memory rounded to 2 bytes per element (default "f32"; DESIGN.md
     §3b: results are those of the f32 index on the rounded points; "f16" refuses values that round to infinity, |x| >= 65520).
+  * `Config.storage = "q8"` keeps them as one byte per element on a grid of each point's own (DESIGN.md §3c: results are those of
+    the f32 index on the dequantised points; points with a NaN or infinite value, or whose grid would overflow f32, are refused).
     The file holds the points widened to f32, so `Hnsw.load / HnswMap.load(..., storage=)` take the storage too.
 """
 import ctypes as C
@@ -45,7 +47,7 @@ class Config:
         self.seed = random.getrandbits(64)
         self.heuristic = Heuristic()
         self.metric = "l2sq"  # or "cosine"
-        self.storage = "f32"  # or "bf16", "f16"
+        self.storage = "f32"  # or "bf16", "f16", "q8"
 
     def _params(self):
         kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed, metric=self.metric,
