@@ -990,6 +990,7 @@ GraphView Index::view() const {
     g.n = n;
     g.flags = opt_flags;
     g.codes = d_codes;
+    g.cwords = code_words(nchunks);
     g.cparams = d_cparams;
     g.cstep = code_step;
     g.cerr = code_err;

@@ -51,7 +51,9 @@ struct GraphView {
     uint32_t flags;              // kOpt* tuning switches (never change results)
     uint32_t row_type;           // RowType (= IDB_STORAGE_*): how the rows are stored; arithmetic stays fp32
     // Screening table (DESIGN §2, §4), or null: K1 then fetches every candidate row in full.
-    const uint32_t* codes;       // n rows of nchunks u32: word c holds the 8-bit codes of elements 4c..4c+3 (byte k = element 4c+k)
+    const uint32_t* codes;       // n rows of cwords u32: word c < nchunks holds the 8-bit codes of elements 4c..4c+3 (byte k = element
+                                 // 4c+k); words [nchunks, cwords) are zero
+    uint32_t cwords;             // code_words(nchunks): every code row starts 16-byte aligned
     const float4* cparams;       // 3 x nchunks float4: per element scale, offset, E (x~ = fmaf(code, scale, offset), |x - x~| <= E)
     float cstep;                 // S: the one code step of every element (the scale slots of cparams all hold it)
     float cerr;                  // R >= ||x - x~|| over every stored row, x~_i = offset_i + code_i * S in real arithmetic
@@ -60,6 +62,8 @@ struct GraphView {
     const float2* hdr;
     uint32_t tail;
 };
+// u32 words per screening-table row: nchunks rounded up to 4, so the screen reads a row in 16-byte words (DESIGN §2)
+__host__ __device__ constexpr uint32_t code_words(uint32_t nchunks) { return (nchunks + 3u) & ~3u; }
 
 // ---------------------------------------------------------------------------------------------------------
 // Canonical squared-L2 (DESIGN.md "canonical distance"; the CPU checker restates the same order):
@@ -255,12 +259,14 @@ __device__ __forceinline__ float butterfly_sum(float s) {
 // split by even/odd index), so NB vectors cost NB-1 shuffles instead of 5*NB; the remaining stages are plain.
 // Same add tree as butterfly_sum for every vector.  On return lane l holds the total of vector (l & (NB-1)).
 // kDown: every add rounds toward -inf instead.  u32 partials (the screen's squared code distances) add exactly, in any order.
+// W < 32 (u32 partials only): the sums run over each aligned group of W lanes on its own (offsets below W).
 template <bool kDown>
 __device__ __forceinline__ float fadd_dir(float a, float b) { return kDown ? __fadd_rd(a, b) : __fadd_rn(a, b); }
 template <bool kDown>
 __device__ __forceinline__ uint32_t fadd_dir(uint32_t a, uint32_t b) { return a + b; }
-template <int NB, bool kDown = false, class T = float>
+template <int NB, bool kDown = false, class T = float, int W = 32>
 __device__ __forceinline__ T batch_butterfly(T (&p)[NB], int lane) {
+    static_assert(NB <= W, "one vector per lane of a group at most");
     int off = 1;
 #pragma unroll
     for (int m = NB; m > 1; m >>= 1) {
@@ -274,7 +280,7 @@ __device__ __forceinline__ T batch_butterfly(T (&p)[NB], int lane) {
         off <<= 1;
     }
 #pragma unroll
-    for (int o = NB; o <= 16; o <<= 1) p[0] = fadd_dir<kDown>(p[0], __shfl_xor_sync(kFullMask, p[0], o));
+    for (int o = NB; o < W; o <<= 1) p[0] = fadd_dir<kDown>(p[0], __shfl_xor_sync(kFullMask, p[0], o));
     return p[0];
 }
 
@@ -846,7 +852,9 @@ __device__ __forceinline__ float screen_finish(float lb) {
     return b > kScreenFloor ? b : 0.f;
 }
 // The query side of the bound: this lane's codes qc (word j = elements 4c..4c+3 of chunk c = lane + 32 j, packed as the table's
-// words) and slack = (r_q + R) rounded up.  Computed once per layer; the retry pass re-runs the layers, so it recomputes it.
+// words; 0 past nchunks) and slack = (r_q + R) rounded up.  Computed once per layer; the retry pass re-runs the layers, so it
+// recomputes it.  screen_slice hands a lane the words the screen's layout (below) reads: kept one word per lane here, the codes
+// hold CH registers across K1's layer instead of 4 CH, for 4 CH shuffles per screen call.
 template <int CH>
 struct ScreenQuery {
     uint32_t qc[CH];
@@ -882,62 +890,95 @@ __device__ __forceinline__ float screen_bound_of(const GraphView& g, uint32_t D,
     const float t = fmaxf(__fsub_rd(__fmul_rd(g.cstep, __fsqrt_rd(__uint2float_rd(D))), slack), 0.f);  // NaN slack: 0
     return screen_finish(__fmul_rd(t, t));
 }
-// acc + sum over this lane's four elements of (qc - c)^2: one VABSDIFF4 and one IDP.4A per code word.
+// acc + sum over a code word's four elements of (qc - c)^2: one VABSDIFF4 and one IDP.4A.
 __device__ __forceinline__ uint32_t screen_word(uint32_t qc, uint32_t w, uint32_t acc) {
     const uint32_t d = __vabsdiffu4(w, qc);
     return __dp4a(d, d, acc);
 }
+// ... over the sixteen elements of a 16-byte word: one IDP.4A chain.
+__device__ __forceinline__ uint32_t screen_words(const uint4& qc, const uint4& w, uint32_t acc) {
+    return screen_word(qc.w, w.w, screen_word(qc.z, w.z, screen_word(qc.y, w.y, screen_word(qc.x, w.x, acc))));
+}
+// The screen's layout (DESIGN §4): a code row is read by a group of eight lanes, lane l taking the 16-byte words 4 (l & 7) + 32 j
+// (j < CH) with one LDG.128 each, so each load instruction of the warp covers four rows.  D is an exact u32, so its adds give the same
+// D in any order and on any lane: this layout need not follow the canonical distance's.  A lane holds screen_slots<CH>() rows (slots)
+// of a batch: <= 32 code words in flight.
 template <int CH>
-__device__ __forceinline__ constexpr int screen_rows() { return CH == 1 ? 32 : CH == 2 ? 16 : CH <= 4 ? 8 : 2; }  // code words in flight <= 32
+__device__ __forceinline__ constexpr int screen_slots() { return CH == 1 ? 8 : CH == 2 ? 4 : CH <= 4 ? 2 : 1; }
+// The query's words of the lane's slice: qc[j] = words 4 (lane & 7) + 32 j .. +3.  Warp-uniform call.
+template <int CH>
+__device__ __forceinline__ void screen_slice(uint4 (&qc)[CH], const ScreenQuery<CH>& sq, int lane) {
+    const int src = 4 * (lane & 7);
+#pragma unroll
+    for (int j = 0; j < CH; ++j)
+        qc[j] = make_uint4(__shfl_sync(kFullMask, sq.qc[j], src), __shfl_sync(kFullMask, sq.qc[j], src + 1),
+                           __shfl_sync(kFullMask, sq.qc[j], src + 2), __shfl_sync(kFullMask, sq.qc[j], src + 3));
+}
+// The lane's code words of one row: 16-byte word j of a row lies past cwords (it is the next row's) unless cok[j].
+template <int CH, bool kFull>
+struct ScreenLane {
+    const char* base;    // g.codes + 16 (lane & 7) bytes
+    uint32_t row_bytes;  // 4 cwords
+    bool cok[CH];
+    __device__ __forceinline__ ScreenLane(const GraphView& g, int lane) {
+        // The base address and the row stride stay in registers (as in batch_distances_impl): each row address is then ONE IMAD.WIDE,
+        // where re-reading g.codes / g.cwords for every predicated row cost about a dozen instructions per row.
+        base = reinterpret_cast<const char*>(g.codes) + 16 * (lane & 7);
+        asm volatile("" : "+l"(base));
+        row_bytes = kFull ? 128u * CH : g.cwords * 4u;
+        if (!kFull) asm volatile("" : "+r"(row_bytes));
+#pragma unroll
+        for (int j = 0; j < CH; ++j) cok[j] = kFull || (uint32_t)(4 * (lane & 7) + 32 * j) < g.cwords;
+    }
+    __device__ __forceinline__ void load(uint4 (&w)[CH], uint32_t pid, bool ok) const {
+        const char* row = base + (size_t)pid * row_bytes;
+#pragma unroll
+        for (int j = 0; j < CH; ++j) w[j] = (ok && cok[j]) ? __ldg(reinterpret_cast<const uint4*>(row + 128 * j)) : make_uint4(0u, 0u, 0u, 0u);
+    }
+};
 // Drops the candidates in cpid[0, n_new) whose bound exceeds fdist (the distance of the ef-th key of nearest) and compacts the rest,
 // in row order, to the front of cpid.  Returns how many are left.  Warp-uniform call.
+// A batch is NS = 4 NSL rows; group grp = lane >> 3 holds rows b0 + NSL grp + i in its slots i < NSL.  After the eight-lane
+// reduction lane l holds row b0 + NSL (l >> 3) + (l & (NSL - 1)) (row b0 + l at NSL = 8), and only lanes with l & 7 < NSL vote, so
+// the ballot keeps the survivors in row order.
 template <int CH, bool kFull>
 __device__ __forceinline__ uint32_t screen_candidates(WarpState& s, const GraphView& g, const ScreenQuery<CH>& sq, uint32_t n_new,
                                                       float fdist, int lane) {
     uint32_t* cpid = s.cpid;
-    constexpr int NS = screen_rows<CH>();
-    bool cok[CH];
-#pragma unroll
-    for (int j = 0; j < CH; ++j) cok[j] = kFull || (uint32_t)(lane + 32 * j) < g.nchunks;
-    // The lane's base address and the row stride stay in registers (as in batch_distances_impl): each row address is then ONE
-    // IMAD.WIDE, where re-reading g.codes / g.nchunks for every predicated row cost about a dozen instructions per row.
-    const char* lane_codes = reinterpret_cast<const char*>(g.codes + lane);
-    asm volatile("" : "+l"(lane_codes));
-    uint32_t row_bytes = kFull ? 32u * CH * 4u : g.nchunks * 4u;
-    if (!kFull) asm volatile("" : "+r"(row_bytes));
+    constexpr int NSL = screen_slots<CH>(), NS = 4 * NSL;
+    const ScreenLane<CH, kFull> sl(g, lane);
+    uint4 qc[CH];
+    screen_slice<CH>(qc, sq, lane);
+    const uint32_t first = NSL * (uint32_t)(lane >> 3), sub = lane & 7;  // this group's first slot row, this lane's place in it
     uint32_t kept = 0;
 #pragma unroll 1
     for (uint32_t b0 = 0; b0 < n_new; b0 += NS) {
-        const uint32_t nb = n_new - b0;
         IDB_PHASE_COUNT(s, kPhScreenBatches, 1u);
-        uint32_t w[NS][CH];
+        // Every slot is loaded and reduced, also in the last, part-filled batch: a warp-uniform skip of the slots no group has a row
+        // in split the batch into blocks, and the headline cell spilled.
+        uint4 w[NSL][CH];
 #pragma unroll
-        for (int i = 0; i < NS; ++i) {
-            const bool ok = (uint32_t)i < nb;
-            const char* row = lane_codes + (size_t)cpid[b0 + i] * row_bytes;  // (entries past n_new are stale ids: never loaded)
-#pragma unroll
-            for (int j = 0; j < CH; ++j) w[i][j] = (ok && cok[j]) ? __ldg(reinterpret_cast<const uint32_t*>(row + 128 * j)) : 0u;
-        }
+        for (int i = 0; i < NSL; ++i) sl.load(w[i], cpid[b0 + first + i], b0 + first + i < n_new);  // (past n_new: stale ids, not loaded)
 #ifdef IDB_K1_PHASES
         {
             uint32_t x = 0;
 #pragma unroll
-            for (int i = 0; i < NS; ++i)
+            for (int i = 0; i < NSL; ++i)
 #pragma unroll
-                for (int j = 0; j < CH; ++j) x ^= w[i][j];
+                for (int j = 0; j < CH; ++j) x ^= w[i][j].x ^ w[i][j].y ^ w[i][j].z ^ w[i][j].w;
             k1_phase_wait(s, x);
             IDB_PHASE(s, kPhScreenLoad);
         }
 #endif
-        const uint32_t mine = (uint32_t)lane < (uint32_t)NS && (uint32_t)lane < nb ? cpid[b0 + lane] : kInvalid;
-        uint32_t p[NS];
+        const uint32_t mine = sub < (uint32_t)NSL && b0 + first + sub < n_new ? cpid[b0 + first + sub] : kInvalid;
+        uint32_t p[NSL];
 #pragma unroll
-        for (int i = 0; i < NS; ++i) p[i] = 0u;
+        for (int i = 0; i < NSL; ++i) {
+            p[i] = 0u;
 #pragma unroll
-        for (int j = 0; j < CH; ++j)
-#pragma unroll
-            for (int i = 0; i < NS; ++i) p[i] = screen_word(sq.qc[j], w[i][j], p[i]);
-        const float bound = screen_bound_of(g, batch_butterfly<NS>(p, lane), sq.slack);  // lane l: row b0 + (l & (NS - 1))
+            for (int j = 0; j < CH; ++j) p[i] = screen_words(qc[j], w[i][j], p[i]);
+        }
+        const float bound = screen_bound_of(g, batch_butterfly<NSL, false, uint32_t, 8>(p, lane), sq.slack);
         const bool keep = mine != kInvalid && !(bound > fdist);
         const uint32_t m = __ballot_sync(kFullMask, keep);
         __syncwarp();  // every lane has read this batch's ids before any is overwritten (writes go to [kept, b0 + NS))

@@ -219,7 +219,8 @@ struct Index {
     const uint32_t** d_upper_ptrs = nullptr;   // device copy of the pointer table
     uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map), cap entries
     bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
-    // Screening table of the stored rows (DESIGN §2, §4): n x nchunks u32 of 8-bit codes + 3 x nchunks float4 (scale, offset, E),
+    // Screening table of the stored rows (DESIGN §2, §4): n x code_words(nchunks) u32 of 8-bit codes (zero padded to a multiple of
+    // 16 bytes) + 3 x nchunks float4 (scale, offset, E),
     // one code step for every element and the bound on every row's coding error (GraphView::cstep / cerr).
     // Null when screening is off (IDB_SCREEN=0), the index is empty, or a stored value is not finite.
     uint32_t* d_codes = nullptr;

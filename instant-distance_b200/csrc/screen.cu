@@ -69,8 +69,9 @@ __device__ __forceinline__ float code_of_value(float x, float offset, float step
     return step > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(x, offset), step)), 0.f), 255.f) : 0.f;
 }
 
-__global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint64_t rows_per_block, float* prm,
-                                   const uint32_t* step, unsigned char* codes) {
+// codes: rows of cstride bytes (4 code_words(nchunks)); the bytes past stride are zeroed beforehand.
+__global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint32_t cstride, uint64_t rows_per_block,
+                                   float* prm, const uint32_t* step, unsigned char* codes) {
     const float S = __uint_as_float(*step);
     if (blockIdx.x == 0)
         for (uint32_t e = threadIdx.x; e < stride; e += blockDim.x) prm[e] = S;
@@ -82,7 +83,7 @@ __global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t 
         for (uint64_t r = r0; r < r1; ++r) {
             const float x = stored_at(pts, row_type, r * stride + e);
             const float c = code_of_value(x, offset, S);
-            codes[r * stride + e] = (unsigned char)c;
+            codes[r * cstride + e] = (unsigned char)c;
             const float xt = __fmaf_rn(c, S, offset);  // x~ of the per-element float bound
             err = fmaxf(err, __fsub_ru(fmaxf(x, xt), fminf(x, xt)));
         }
@@ -95,14 +96,14 @@ __global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t 
 __global__ void code_row_err_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t nchunks, const float* prm,
                                     const uint32_t* step, const uint32_t* codes, uint32_t* err_max) {
     const float S = __uint_as_float(*step);
-    const uint32_t stride = nchunks * 4;
+    const uint32_t stride = nchunks * 4, cwords = code_words(nchunks);
     const int lane = threadIdx.x & 31;
     const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
     float worst = 0.f;
     for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < n; r += warps) {
         float acc = 0.f;
         for (uint32_t c = lane; c < nchunks; c += 32) {
-            const uint32_t w = codes[r * nchunks + c];
+            const uint32_t w = codes[r * cwords + c];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const uint32_t e = 4 * c + k;
@@ -119,7 +120,8 @@ __global__ void code_row_err_kernel(const void* pts, uint32_t row_type, uint64_t
 }
 
 // One warp per (query, row) pair: the screen's bound (what K1 compares with the furthest distance) and the canonical distance.
-// The same helpers as K1's screen_candidates: screen_query, screen_word, batch_butterfly, screen_bound_of.
+// The same helpers and layout as K1's screen_candidates (screen_query, screen_slice, ScreenLane, screen_words, batch_butterfly over eight lanes,
+// screen_bound_of): each group of eight lanes reduces the row on its own, as one K1 slot does.
 template <int CH, class RT>
 __global__ void screen_bound_kernel(GraphView g, const float4* queries, const uint32_t* pairs, uint64_t npairs, float* out_bound,
                                     float* out_dist) {
@@ -134,13 +136,13 @@ __global__ void screen_bound_kernel(GraphView g, const float4* queries, const ui
     const float dist = butterfly_sum(lane_partial<CH>(q.r, x));
     ScreenQuery<CH> sq;
     screen_query<CH>(sq, g, q.r, lane);
+    uint4 qc[CH], cw[CH];
+    screen_slice<CH>(qc, sq, lane);
+    ScreenLane<CH, false>(g, lane).load(cw, pid, true);
     uint32_t p[1] = {0u};
 #pragma unroll
-    for (int j = 0; j < CH; ++j) {
-        const uint32_t c = lane + 32 * j;
-        p[0] = screen_word(sq.qc[j], c < g.nchunks ? g.codes[(size_t)pid * g.nchunks + c] : 0u, p[0]);
-    }
-    const float bound = screen_bound_of(g, batch_butterfly<1>(p, lane), sq.slack);
+    for (int j = 0; j < CH; ++j) p[0] = screen_words(qc[j], cw[j], p[0]);
+    const float bound = screen_bound_of(g, batch_butterfly<1, false, uint32_t, 8>(p, lane), sq.slack);
     if (lane == 0) {
         out_bound[w] = bound;
         out_dist[w] = dist;
@@ -166,14 +168,15 @@ idb_status Index::build_codes() {
     d_codes = nullptr;
     d_cparams = nullptr;
     if (!screen || n == 0 || row_type == kRowQ8) return IDB_OK;  // DESIGN §3c: q8 rows are one byte per element already
-    const uint32_t stride = nchunks * 4;
+    const uint32_t stride = nchunks * 4, cstride = code_words(nchunks) * 4;
     const void* pts = rows();
     const unsigned grid = (unsigned)std::min<uint64_t>((n + 63) / 64, (uint64_t)num_sms * 8);
     const uint64_t rows_per_block = (n + grid - 1) / grid;
     uint32_t* tmp = nullptr;  // [0, stride) min, [stride, 2 stride) max, [2 stride] non-finite flag, [2 stride + 1] S, [2 stride + 2] R
     CUDA_TRY(cudaMalloc(&tmp, (2 * (size_t)stride + 3) * 4));
     cudaError_t e = cudaMalloc(&d_cparams, 3 * (size_t)stride * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&d_codes, n * (size_t)stride);
+    if (e == cudaSuccess) e = cudaMalloc(&d_codes, n * (size_t)cstride);
+    if (e == cudaSuccess && cstride != stride) e = cudaMemsetAsync(d_codes, 0, n * (size_t)cstride, stream);  // the padding words
     if (e == cudaSuccess) e = fill_u32(tmp, stride, 0xFFFFFFFFu, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(tmp + stride, 0, ((size_t)stride + 3) * 4, stream);
     if (e == cudaSuccess) {
@@ -188,7 +191,7 @@ idb_status Index::build_codes() {
         float* prm = reinterpret_cast<float*>(d_cparams);
         uint32_t* step = tmp + 2 * stride + 1;
         code_params_kernel<<<(stride + 127) / 128, 128, 0, stream>>>(tmp, tmp + stride, stride, prm, step);
-        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, rows_per_block, prm, step,
+        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, cstride, rows_per_block, prm, step,
                                                      reinterpret_cast<unsigned char*>(d_codes));
         code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(pts, row_type, n, nchunks, prm, step, d_codes, step + 1);
         e = cudaGetLastError();
