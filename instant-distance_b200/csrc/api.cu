@@ -78,138 +78,6 @@ cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, ui
     return cudaGetLastError();
 }
 
-// f32 -> bf16 / fp16 (round to nearest even) and back (exact), element-wise over the padded row matrix
-__global__ void narrow_bf16_kernel(const float* src, uint16_t* dst, size_t n) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t b = __float_as_uint(src[i]);
-        uint32_t r;
-        if ((b & 0x7fffffffu) > 0x7f800000u) r = (b >> 16) | 0x40u;           // NaN stays NaN
-        else r = (b + 0x7fffu + ((b >> 16) & 1u)) >> 16;                       // RNE
-        dst[i] = (uint16_t)r;
-    }
-}
-__global__ void widen_bf16_kernel(const uint16_t* src, float* dst, size_t n) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        dst[i] = __uint_as_float((uint32_t)src[i] << 16);
-}
-// cvt.rn.f16.f32 is RNE with subnormal results kept and overflow to +-inf (refused beforehand by check_f16_range); a NaN keeps its sign
-// and top payload bits, quieted (what the x86 F16C conversion and numpy give for a quiet NaN).
-__global__ void narrow_f16_kernel(const float* src, uint16_t* dst, size_t n) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float x = src[i];
-        const uint32_t b = __float_as_uint(x);
-        unsigned short h;
-        if ((b & 0x7fffffffu) > 0x7f800000u) h = (unsigned short)(((b >> 16) & 0x8000u) | 0x7e00u | ((b >> 13) & 0x3ffu));
-        else asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
-        dst[i] = h;
-    }
-}
-// Exact, and a NaN keeps its sign and payload (cvt.f32.f16 would return the canonical NaN), so an export or a save gives back the
-// f32 value of every stored bit pattern.
-__global__ void widen_f16_kernel(const uint16_t* src, float* dst, size_t n) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t h = src[i];
-        dst[i] = (h & 0x7fffu) > 0x7c00u ? __uint_as_float(((h & 0x8000u) << 16) | 0x7f800000u | ((h & 0x3ffu) << 13))
-                                         : widen_f16x2(h).x;
-    }
-}
-// The smallest flat index of a finite element that rounds to +-inf in fp16 (|x| >= 65520, halfway to the next binade past 65504).
-__global__ void f16_overflow_kernel(const float* src, size_t n, unsigned long long* first) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float x = fabsf(src[i]);
-        if (x >= 65520.f && x <= 3.402823466e38f) atomicMin(first, (unsigned long long)i);
-    }
-}
-
-// q8 rows (DESIGN §3c).  The grid of a row x of `dim` finite f32 values, in f64, where every step below is exact (x * 2^-e is a
-// power-of-two scaling of an f32):
-//   A = max |x_i|;  A == 0: e = -149, b = 0.  Else e_lo = max(-149, ilogb(A) - 23) and e = the smallest e >= e_lo with
-//   ceil(max x / 2^e) - floor(min x / 2^e) <= 255;  b = floor(min x / 2^e);  c_i = rint(x_i / 2^e) - b in [0, 255].
-// Element i is (b + c_i) 2^e, |b + c_i| < 2^24, so it and the header {o, s} = {b 2^e, 2^e} are exact f32 unless they overflow.
-struct Q8Grid {
-    int e;
-    double b, scale;  // scale = 2^-e
-};
-__device__ __forceinline__ double pow2(int k) { return __hiloint2double((1023 + k) << 20, 0); }  // 2^k, -1022 <= k <= 1023
-__device__ __forceinline__ Q8Grid q8_grid(float mn, float mx) {
-    Q8Grid g;
-    const float A = fmaxf(fabsf(mn), fabsf(mx));
-    if (A == 0.f) {
-        g.e = -149;
-        g.b = 0.0;
-        g.scale = pow2(149);
-        return g;
-    }
-    int e = max(-149, ilogbf(A) - 23);
-    while (ceil((double)mx * pow2(-e)) - floor((double)mn * pow2(-e)) > 255.0) ++e;  // at most ~25 steps
-    g.e = e;
-    g.scale = pow2(-e);
-    g.b = floor((double)mn * g.scale);
-    return g;
-}
-// The row's min and max over its first dim elements (one warp per row; every lane ends with both) and whether all are finite.
-__device__ __forceinline__ bool q8_row_range(const float* x, uint32_t dim, int lane, float* mn, float* mx) {
-    float lo = INFINITY, hi = -INFINITY;
-    bool fin = true;
-    for (uint32_t i = lane; i < dim; i += 32) {
-        const float v = x[i];
-        fin = fin && isfinite(v);
-        lo = fminf(lo, v);
-        hi = fmaxf(hi, v);
-    }
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-        lo = fminf(lo, __shfl_xor_sync(kFullMask, lo, o));
-        hi = fmaxf(hi, __shfl_xor_sync(kFullMask, hi, o));
-    }
-    *mn = lo;
-    *mx = hi;
-    return __all_sync(kFullMask, fin);
-}
-// v 2^e is an f32 (not infinite), for an integer |v| < 2^24
-__device__ __forceinline__ bool q8_fits(double v, int e) { return fabs(v) * pow2(e) < 0x1p128; }
-// The smallest flat index (row * stride + element) of an element that refuses its row: a NaN or +-inf, else (a finite row whose
-// header or a dequantised element overflows f32) the first element that overflows, or the row's first minimum when only o does.
-__global__ void check_q8_kernel(const float* rows, uint64_t m, uint32_t stride, uint32_t dim, unsigned long long* first) {
-    const int lane = threadIdx.x & 31;
-    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
-    for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < m; r += warps) {
-        const float* x = rows + r * stride;
-        float mn, mx;
-        if (!q8_row_range(x, dim, lane, &mn, &mx)) {
-            for (uint32_t i = lane; i < dim; i += 32)
-                if (!isfinite(x[i])) atomicMin(first, (unsigned long long)(r * stride + i));
-            continue;
-        }
-        const Q8Grid g = q8_grid(mn, mx);
-        const bool o_ok = q8_fits(g.b, g.e);
-        for (uint32_t i = lane; i < dim; i += 32)
-            if (!q8_fits(rint((double)x[i] * g.scale), g.e) || (!o_ok && x[i] == mn)) atomicMin(first, (unsigned long long)(r * stride + i));
-    }
-}
-// Codes (stride bytes per row, padding codes 0) and headers of m checked rows.  One warp per row.
-__global__ void quantize_q8_kernel(const float* rows, uint64_t m, uint32_t stride, uint32_t dim, uint8_t* codes, float2* hdr) {
-    const int lane = threadIdx.x & 31;
-    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
-    for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; r < m; r += warps) {
-        const float* x = rows + r * stride;
-        float mn, mx;
-        q8_row_range(x, dim, lane, &mn, &mx);
-        const Q8Grid g = q8_grid(mn, mx);
-        for (uint32_t i = lane; i < stride; i += 32)
-            codes[r * stride + i] = i < dim ? (uint8_t)(rint((double)x[i] * g.scale) - g.b) : (uint8_t)0;
-        if (lane == 0) hdr[r] = make_float2((float)(g.b * pow2(g.e)), (float)pow2(g.e));
-    }
-}
-// The dequantised rows: element i < dim is fmaf(c_i, s, o) (exact), the padding 0.
-__global__ void widen_q8_kernel(const uint8_t* codes, const float2* hdr, uint64_t m, uint32_t stride, uint32_t dim, float* dst) {
-    const size_t total = m * stride;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const float2 h = hdr[i / stride];
-        dst[i] = i % stride < dim ? __fmaf_rn((float)codes[i], h.y, h.x) : 0.f;
-    }
-}
-
 // Adjacency sanity check for graphs adopted from outside (idb_index_from_graph_*, idb_index_load): every entry must be
 // INVALID or a PointId below `limit`; otherwise the traversal would read out of bounds.
 __global__ void validate_rows_kernel(const uint32_t* rows, size_t count, uint32_t limit, uint32_t* bad) {
@@ -787,200 +655,16 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, 
     return IDB_OK;
 }
 
-cudaError_t narrow_elems(const float* src, uint16_t* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st) {
-    if (count == 0) return cudaSuccess;
-    if (type == kRowF16) narrow_f16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
-    else narrow_bf16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
-    return cudaGetLastError();
-}
-cudaError_t widen_elems(const uint16_t* src, float* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st) {
-    if (count == 0) return cudaSuccess;
-    if (type == kRowF16) widen_f16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
-    else widen_bf16_kernel<<<num_sms * 8, 256, 0, st>>>(src, dst, count);
-    return cudaGetLastError();
-}
-
-idb_status check_f16_range(const float* d_rows, uint64_t m, uint32_t nchunks, const uint32_t* input_row, uint64_t row0, int num_sms,
-                           cudaStream_t st) {
-    const size_t stride = (size_t)nchunks * 4, total = m * stride;
-    if (total == 0) return IDB_OK;
-    unsigned long long* d_first = nullptr;
-    unsigned long long first = ~0ull;
-    CUDA_TRY(cudaMalloc(&d_first, 8));
-    cudaError_t e = cudaMemcpyAsync(d_first, &first, 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        f16_overflow_kernel<<<num_sms * 8, 256, 0, st>>>(d_rows, total, d_first);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&first, d_first, 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    float x = 0.f;
-    if (e == cudaSuccess && first != ~0ull) e = cudaMemcpy(&x, d_rows + first, 4, cudaMemcpyDeviceToHost);
-    cudaFree(d_first);
-    CUDA_TRY(e);
-    if (first == ~0ull) return IDB_OK;
-    const uint64_t r = first / stride;
-    return fail(IDB_ERR_INVALID_ARG, "fp16 storage: row %llu, element %llu is %g, which rounds to infinity in fp16 (|x| >= 65520)",
-                (unsigned long long)(input_row ? input_row[r] : row0 + r), (unsigned long long)(first % stride), (double)x);
-}
-
-idb_status check_q8_rows(const float* d_rows, uint64_t m, uint32_t nchunks, uint32_t dim, const uint32_t* input_row, uint64_t row0,
-                         int num_sms, cudaStream_t st) {
-    const size_t stride = (size_t)nchunks * 4;
-    if (m == 0) return IDB_OK;
-    unsigned long long* d_first = nullptr;
-    unsigned long long first = ~0ull;
-    CUDA_TRY(cudaMalloc(&d_first, 8));
-    cudaError_t e = cudaMemcpyAsync(d_first, &first, 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        check_q8_kernel<<<num_sms * 8, 256, 0, st>>>(d_rows, m, (uint32_t)stride, dim, d_first);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&first, d_first, 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    float x = 0.f;
-    if (e == cudaSuccess && first != ~0ull) e = cudaMemcpy(&x, d_rows + first, 4, cudaMemcpyDeviceToHost);
-    cudaFree(d_first);
-    CUDA_TRY(e);
-    if (first == ~0ull) return IDB_OK;
-    const unsigned long long r = input_row ? input_row[first / stride] : row0 + first / stride, i = first % stride;
-    if (!std::isfinite(x))
-        return fail(IDB_ERR_INVALID_ARG, "q8 storage: row %llu, element %llu is %g; q8 rows must be finite", r, i, (double)x);
-    return fail(IDB_ERR_INVALID_ARG, "q8 storage: row %llu, element %llu (%g): the row's dequantised values would overflow f32", r, i,
-                (double)x);
-}
-
-cudaError_t quantize_q8(const float* src, uint64_t m, uint32_t nchunks, uint32_t dim, uint8_t* codes, float2* hdr, int num_sms,
-                        cudaStream_t st) {
-    if (m == 0) return cudaSuccess;
-    quantize_q8_kernel<<<num_sms * 8, 256, 0, st>>>(src, m, nchunks * 4, dim, codes, hdr);
-    return cudaGetLastError();
-}
-
-idb_status Index::narrow_points(uint32_t type, const uint32_t* input_row) {
-    if (type == kRowF16) {
-        const idb_status s = check_f16_range(d_points, n, nchunks, input_row, 0, num_sms, stream);
-        if (s != IDB_OK) return s;
-    }
-    if (type == kRowQ8) {
-        const idb_status s = check_q8_rows(d_points, n, nchunks, dim, input_row, 0, num_sms, stream);
-        if (s != IDB_OK) return s;
-    }
-    const size_t total = n * (size_t)nchunks * 4;
-    if (total == 0) { row_type = type; return IDB_OK; }
-    if (type == kRowQ8) {
-        CUDA_TRY(cudaMalloc(&d_points8, cap * (size_t)nchunks * 4));
-        CUDA_TRY(cudaMalloc(&d_hdr, cap * sizeof(float2)));
-        CUDA_TRY(quantize_q8(d_points, n, nchunks, dim, d_points8, d_hdr, num_sms, stream));
-    } else {
-        CUDA_TRY(cudaMalloc(&d_points16, cap * (size_t)nchunks * 4 * 2));
-        CUDA_TRY(narrow_elems(d_points, d_points16, total, type, num_sms, stream));
-    }
+idb_status Index::stage_rows(uint64_t r0, uint64_t m, const uint32_t* global_ids) {
+    CUDA_TRY(fill_u32(d_zero + r0 * 2 * M, m * 2 * M, kInvalid, stream));
+    if (d_id_map) CUDA_TRY(cudaMemcpyAsync(d_id_map + r0, global_ids, m * 4, cudaMemcpyHostToDevice, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
-    cudaFree(d_points);
-    d_points = nullptr;
-    row_type = type;
-    return IDB_OK;
-}
-
-idb_status Index::reserve_rows(uint64_t rows) {
-    if (rows <= cap) return IDB_OK;
-    const uint64_t want = std::max<uint64_t>(rows, 2 * cap);
-    const size_t stride = (size_t)nchunks * 4, width = 2 * (size_t)M;
-    void* pts = nullptr;
-    float2* hdr = nullptr;
-    uint32_t* zero = nullptr;
-    uint32_t* id_map = nullptr;
-    cudaError_t e = cudaMalloc(&pts, want * stride * elem_bytes());
-    if (e == cudaSuccess && row_type == kRowQ8) e = cudaMalloc(&hdr, want * sizeof(float2));
-    if (e == cudaSuccess) e = cudaMalloc(&zero, want * width * 4);
-    if (e == cudaSuccess && d_id_map) e = cudaMalloc(&id_map, want * 4);
-    if (e == cudaSuccess && n) {
-        e = cudaMemcpyAsync(pts, this->rows(), n * stride * elem_bytes(), cudaMemcpyDeviceToDevice, stream);
-        if (e == cudaSuccess && hdr) e = cudaMemcpyAsync(hdr, d_hdr, n * sizeof(float2), cudaMemcpyDeviceToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(zero, d_zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
-        if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(id_map, d_id_map, n * 4, cudaMemcpyDeviceToDevice, stream);
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) {
-        cudaFree(pts);
-        cudaFree(hdr);
-        cudaFree(zero);
-        cudaFree(id_map);
-        CUDA_TRY(e);
-    }
-    cudaFree(d_points);
-    cudaFree(d_points16);
-    cudaFree(d_points8);
-    cudaFree(d_hdr);
-    cudaFree(d_zero);
-    cudaFree(d_id_map);
-    d_points = row_type == kRowF32 ? static_cast<float*>(pts) : nullptr;
-    d_points16 = row_type == kRowBF16 || row_type == kRowF16 ? static_cast<uint16_t*>(pts) : nullptr;
-    d_points8 = row_type == kRowQ8 ? static_cast<uint8_t*>(pts) : nullptr;
-    d_hdr = hdr;
-    d_zero = zero;
-    d_id_map = id_map;
-    cap = want;
-    return IDB_OK;
-}
-
-idb_status Index::stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids) {
-    const size_t stride = (size_t)nchunks * 4;
-    float* tmp = nullptr;  // the rows in the kernel layout, f32
-    CUDA_TRY(cudaMalloc(&tmp, m * stride * 4));
-    cudaError_t e = cudaMemsetAsync(tmp, 0, m * stride * 4, stream);
-    if (e == cudaSuccess) e = cudaMemcpy2DAsync(tmp, stride * 4, rows, dim * 4, dim * 4, m, cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess && metric == kMetricCosine) e = normalize_rows(tmp, stride, tmp, m, dim, nchunks, num_sms, stream);
-    if (e == cudaSuccess && (row_type == kRowF16 || row_type == kRowQ8)) {  // before anything of the index is written; rows named as
-        const idb_status s = row_type == kRowF16 ? check_f16_range(tmp, m, nchunks, nullptr, 0, num_sms, stream)  // the caller numbers them
-                                                 : check_q8_rows(tmp, m, nchunks, dim, nullptr, 0, num_sms, stream);
-        if (s != IDB_OK) {
-            cudaFree(tmp);
-            return s;
-        }
-    }
-    if (e == cudaSuccess && row_type == kRowQ8)  // normalised first, then quantised, as the build does
-        e = quantize_q8(tmp, m, nchunks, dim, d_points8 + r0 * stride, d_hdr + r0, num_sms, stream);
-    else if (e == cudaSuccess && row_type != kRowF32)  // normalised first, then rounded, as the build does
-        e = narrow_elems(tmp, d_points16 + r0 * stride, m * stride, row_type, num_sms, stream);
-    else if (e == cudaSuccess)
-        e = cudaMemcpyAsync(d_points + r0 * stride, tmp, m * stride * 4, cudaMemcpyDeviceToDevice, stream);
-    if (e == cudaSuccess) e = fill_u32(d_zero + r0 * 2 * M, m * 2 * M, kInvalid, stream);
-    if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(d_id_map + r0, global_ids, m * 4, cudaMemcpyHostToDevice, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    cudaFree(tmp);
-    CUDA_TRY(e);
-    return IDB_OK;
-}
-
-idb_status Index::copy_points_f32(float* host_out, uint64_t r0, uint64_t m) {
-    if (m == 0) return IDB_OK;
-    const size_t stride = (size_t)nchunks * 4;
-    if (row_type == kRowF32) {
-        CUDA_TRY(cudaMemcpy2DAsync(host_out, dim * 4, d_points + r0 * stride, stride * 4, dim * 4, m, cudaMemcpyDeviceToHost, stream));
-        CUDA_TRY(cudaStreamSynchronize(stream));
-        return IDB_OK;
-    }
-    float* tmp = nullptr;
-    CUDA_TRY(cudaMalloc(&tmp, m * stride * 4));
-    cudaError_t e = cudaSuccess;
-    if (row_type == kRowQ8) {
-        widen_q8_kernel<<<num_sms * 8, 256, 0, stream>>>(d_points8 + r0 * stride, d_hdr + r0, m, (uint32_t)stride, dim, tmp);
-        e = cudaGetLastError();
-    } else {
-        e = widen_elems(d_points16 + r0 * stride, tmp, m * stride, row_type, num_sms, stream);
-    }
-    if (e == cudaSuccess) e = cudaMemcpy2DAsync(host_out, dim * 4, tmp, stride * 4, dim * 4, m, cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    cudaFree(tmp);
-    CUDA_TRY(e);
     return IDB_OK;
 }
 
 GraphView Index::view() const {
     GraphView g;
-    g.points = static_cast<const char*>(rows());
+    g.points = static_cast<const char*>(d_rows);
     g.row_type = row_type;
     g.nchunks = nchunks;
     g.zero = d_zero;
@@ -1003,9 +687,7 @@ Index::~Index() {
     cudaSetDevice(device);
     for (auto& ln : lanes)
         if (ln.stream) cudaStreamSynchronize(ln.stream);
-    cudaFree(d_points);
-    cudaFree(d_points16);
-    cudaFree(d_points8);
+    cudaFree(d_rows);
     cudaFree(d_hdr);
     cudaFree(d_codes);
     cudaFree(d_cparams);
@@ -1046,9 +728,8 @@ idb_status Index::init_device(int dev) {
     return IDB_OK;
 }
 
-// Upload a graph (host arrays) into HBM.
-idb_status Index::upload(const float* points, uint64_t n_, uint32_t dim_, uint32_t M_, uint32_t ef, const uint32_t* zero,
-                         uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n_) {
+idb_status Index::upload(uint64_t n_, uint32_t dim_, uint32_t M_, uint32_t ef, const uint32_t* zero, uint32_t n_upper,
+                         const uint32_t* const* upper, const uint64_t* upper_n_) {
     // Layer l holds PointIds [0, n_l) (lib.rs:275-281): n >= n_1 >= n_2 >= ... >= 1.  The descent carries ids found on layer l
     // into layer l-1 and seeds PointId 0 on the top layer, so anything else would read adjacency rows out of bounds.
     for (uint32_t l = 0; l < n_upper; ++l) {
@@ -1066,14 +747,6 @@ idb_status Index::upload(const float* points, uint64_t n_, uint32_t dim_, uint32
     if (n == 0) return IDB_OK;
     const size_t stride = (size_t)nchunks * 4;
     if (n > SIZE_MAX / (stride * sizeof(float)) || n > SIZE_MAX / (2 * (size_t)M * 4)) return fail(IDB_ERR_INVALID_ARG, "n * dim overflows size_t");
-    CUDA_TRY(cudaMalloc(&d_points, n * stride * sizeof(float)));
-    if (stride == dim) {
-        CUDA_TRY(cudaMemcpyAsync(d_points, points, n * stride * sizeof(float), cudaMemcpyHostToDevice, stream));
-    } else {
-        CUDA_TRY(cudaMemsetAsync(d_points, 0, n * stride * sizeof(float), stream));
-        CUDA_TRY(cudaMemcpy2DAsync(d_points, stride * sizeof(float), points, dim * sizeof(float), dim * sizeof(float), n,
-                                   cudaMemcpyHostToDevice, stream));
-    }
     CUDA_TRY(cudaMalloc(&d_zero, n * 2 * (size_t)M * 4));
     if (zero) CUDA_TRY(cudaMemcpyAsync(d_zero, zero, n * 2 * (size_t)M * 4, cudaMemcpyHostToDevice, stream));
     std::vector<const uint32_t*> ptrs;
@@ -1154,12 +827,14 @@ idb_status adopt_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M
         ix = new (std::nothrow) Index();
         if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
         ix->metric = metric;
+        ix->row_type = storage;
         idb_status s = ix->init_device(device);
-        if (s == IDB_OK) s = ix->upload(points, n, dim, M, ef_search, zero, n_upper, upper, upper_n);
+        if (s == IDB_OK) s = ix->upload(n, dim, M, ef_search, zero, n_upper, upper, upper_n);
         return s;
     }();
     if (st == IDB_ERR_INVALID_ARG && from_file) st = IDB_ERR_FORMAT;
-    if (st == IDB_OK && storage != IDB_STORAGE_F32) st = ix->narrow_points(storage, nullptr);
+    if (st == IDB_OK)  // the rows as given; fp16 / q8 rows beyond the storage's range are refused, named by their row in the call
+        st = ix->put_rows(0, n, nullptr, [&](float* dst) { return ix->copy_rows_in(dst, points, n); });
     if (st == IDB_OK) st = ix->build_codes();
     if (st != IDB_OK) {
         delete ix;

@@ -319,10 +319,7 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     ix->M = M;
     ix->ef_search = p.ef_search;
     ix->nchunks = (dim + 3) / 4;
-    if (n == 0) {  // lib.rs:224-234; the storage is recorded for the rows a later insert adds
-        ix->row_type = p.storage;
-        return IDB_OK;
-    }
+    if (n == 0) return IDB_OK;  // lib.rs:224-234
     cudaStream_t st = ix->stream;
     const uint32_t cap = 2 * M;
     const size_t stride = (size_t)ix->nchunks * 4;
@@ -344,27 +341,26 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
     }
 
     // ---- device arrays ----------------------------------------------------------------------------------------
-    {
+    ix->cap = n;
+    idb_status s = ix->put_rows(0, n, order.data(), [&](float* dst) {  // refusals name the caller's row, order[PointId]
         float* d_rows = nullptr;
         uint32_t* d_order = nullptr;
-        CUDA_TRY(cudaMalloc(&ix->d_points, n * stride * sizeof(float)));
-        ix->cap = n;
-        CUDA_TRY(cudaMalloc(&d_rows, n * (size_t)dim * sizeof(float)));
-        CUDA_TRY(cudaMalloc(&d_order, n * sizeof(uint32_t)));
-        CUDA_TRY(cudaMemcpyAsync(d_rows, rows, n * (size_t)dim * sizeof(float), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_order, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        gather_rows_kernel<<<ix->num_sms * 8, 256, 0, st>>>(d_rows, d_order, ix->d_points, n, dim, (uint32_t)stride);
-        CUDA_TRY(cudaGetLastError());
-        if (ix->metric == kMetricCosine)  // DESIGN §3a: a cosine index stores the normalised rows (bf16 / fp16: normalised, then rounded)
-            CUDA_TRY(normalize_rows(ix->d_points, stride, ix->d_points, n, dim, ix->nchunks, ix->num_sms, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        cudaError_t e = cudaMalloc(&d_rows, n * (size_t)dim * sizeof(float));
+        if (e == cudaSuccess) e = cudaMalloc(&d_order, n * sizeof(uint32_t));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_rows, rows, n * (size_t)dim * sizeof(float), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_order, order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) {
+            gather_rows_kernel<<<ix->num_sms * 8, 256, 0, st>>>(d_rows, d_order, dst, n, dim, (uint32_t)stride);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess && ix->metric == kMetricCosine)  // DESIGN §3a: a cosine index stores the normalised rows
+            e = normalize_rows(dst, stride, dst, n, dim, ix->nchunks, ix->num_sms, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
         cudaFree(d_rows);
         cudaFree(d_order);
-    }
-    if (p.storage != IDB_STORAGE_F32) {  // fp16 / q8: rows beyond the storage's range are refused here, named by their input row
-        idb_status sb = ix->narrow_points(p.storage, order.data());
-        if (sb != IDB_OK) return sb;
-    }
+        return e;
+    });
+    if (s != IDB_OK) return s;
     CUDA_TRY(cudaMalloc(&ix->d_zero, n * (size_t)cap * 4));
     CUDA_TRY(fill_u32(ix->d_zero, n * (size_t)cap, kInvalid, st));
     std::vector<const uint32_t*> ptrs;
@@ -422,7 +418,14 @@ idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_para
     if (m == 0) return IDB_OK;
     // ---- storage: grow (copying the first n0 rows), then stage the new rows behind them; nothing below n0 changes -------------
     idb_status s = ix->reserve_rows(n1);
-    if (s == IDB_OK) s = ix->stage_rows(rows, n0, m, global_ids);
+    if (s == IDB_OK)
+        s = ix->put_rows(n0, m, nullptr, [&](float* dst) {  // refusals name the row within the call
+            cudaError_t e = ix->copy_rows_in(dst, rows, m);
+            if (e == cudaSuccess && ix->metric == kMetricCosine)
+                e = normalize_rows(dst, (size_t)ix->nchunks * 4, dst, m, ix->dim, ix->nchunks, ix->num_sms, ix->stream);
+            return e;
+        });
+    if (s == IDB_OK) s = ix->stage_rows(n0, m, global_ids);
     if (s != IDB_OK) return s;
     uint32_t max_batch = 0, growth = 0;
     batch_schedule(p, &max_batch, &growth);
@@ -485,6 +488,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
     auto* ix = new (std::nothrow) Index();
     if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
     ix->metric = metric;
+    ix->row_type = params->storage;
     idb_status st = ix->init_device(params->device);
     if (st == IDB_OK) {
         std::lock_guard<std::mutex> lk(ix->mu);

@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <functional>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -194,6 +195,28 @@ struct Lane {
     void free_all();
 };
 
+// The stored rows as the export, the save and the screening table read them (Index::stored, rows.cu); K1, the build and the exact scan
+// read them through the row traits of hnsw_device.cuh instead.
+struct StoredRows {
+    const void* rows;      // cap x stride elements of `type`
+    const float2* hdr;     // q8 row headers {o, s}
+    uint32_t type, stride, dim;
+};
+// Element e (< stride) of stored row r, exactly as f32: bf16 by the 16-bit shift; fp16 by cvt.f32.f16, except that a NaN keeps its
+// sign and payload (cvt.f32.f16 would return the canonical NaN), so an export or a save gives back the f32 value of every stored
+// bit pattern; q8 as fmaf(c, s, o), and 0 past dim.
+__device__ __forceinline__ float stored_elem(const StoredRows& s, uint64_t r, uint32_t e) {
+    const size_t i = r * s.stride + e;
+    if (s.type == kRowF32) return static_cast<const float*>(s.rows)[i];
+    if (s.type == kRowQ8) {
+        const float2 h = s.hdr[r];
+        return e < s.dim ? __fmaf_rn((float)static_cast<const uint8_t*>(s.rows)[i], h.y, h.x) : 0.f;
+    }
+    const uint32_t h = static_cast<const uint16_t*>(s.rows)[i];
+    if (s.type == kRowBF16) return __uint_as_float(h << 16);
+    return (h & 0x7fffu) > 0x7c00u ? __uint_as_float(((h & 0x8000u) << 16) | 0x7f800000u | ((h & 0x3ffu) << 13)) : widen_f16x2(h).x;
+}
+
 struct Index {
     int device = 0;
     int num_sms = 132;
@@ -207,11 +230,9 @@ struct Index {
     std::atomic<uint64_t> n{0};                // written by an insert while other threads may read it (searches take a lane first)
     uint64_t cap = 0;                          // rows allocated for points, zero and the id map (>= n; grows by doubling on insert)
     uint32_t dim = 0, nchunks = 0, M = 32, ef_search = 100;
-    float* d_points = nullptr;                 // cap x nchunks*4 f32 (PointId order); null when the rows are stored narrower
-    uint16_t* d_points16 = nullptr;            // cap x nchunks*4 bf16 or fp16 (row_type kRowBF16 / kRowF16), else null
-    uint8_t* d_points8 = nullptr;              // cap x nchunks*4 q8 codes (row_type kRowQ8), else null
+    void* d_rows = nullptr;                    // cap x nchunks*4 elements of row_type (PointId order): f32, bf16 / fp16, or q8 codes
     float2* d_hdr = nullptr;                   // cap q8 row headers {o, s} (DESIGN §3c), else null
-    uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as
+    uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as; set when the index is created
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
     uint32_t* d_zero = nullptr;                // cap x 2M (rows past n: INVALID)
     std::vector<uint32_t*> d_upper;            // [l-1] -> n_l x M
@@ -249,27 +270,29 @@ struct Index {
 
     ~Index();
     idb_status init_device(int dev);
-    idb_status upload(const float* points, uint64_t n, uint32_t dim, uint32_t M, uint32_t ef, const uint32_t* zero,
-                      uint32_t n_upper, const uint32_t* const* upper, const uint64_t* upper_n);
+    // The graph of an index of n rows (cap = n): layer sizes checked, zero and upper allocated (and copied when given), adjacency
+    // entries checked.  The rows are put in by the caller (put_rows).
+    idb_status upload(uint64_t n, uint32_t dim, uint32_t M, uint32_t ef, const uint32_t* zero, uint32_t n_upper,
+                      const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
-    uint32_t elem_bytes() const { return row_type == kRowF32 ? 4u : row_type == kRowQ8 ? 1u : 2u; }
-    const void* rows() const {
-        return row_type == kRowF32 ? static_cast<const void*>(d_points)
-               : row_type == kRowQ8 ? static_cast<const void*>(d_points8) : static_cast<const void*>(d_points16);
-    }
-    // d_points (f32) -> d_points16 in `type` (kRowBF16 / kRowF16), or d_points8 + d_hdr (kRowQ8), freeing d_points.  fp16 / q8:
-    // refused (IDB_ERR_INVALID_ARG, the index unchanged) when a row is beyond the storage's range (check_f16_range, check_q8_rows);
-    // the message names the caller's row, input_row[PointId] when given.
-    idb_status narrow_points(uint32_t type, const uint32_t* input_row);
-    // Storage for at least `rows` points: points, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
+    // ---- the row storage (rows.cu) ----
+    StoredRows stored() const;
+    // Rows [r0, r0 + m) (r0 >= n, r0 + m <= cap) of the store.  fill(dst) writes them as nchunks * 4 f32 per row, zero padded (the
+    // kernel layout), into the store itself for f32 rows, else into a staging buffer.  Then the storage's refusal (fp16, q8) runs
+    // over the staged rows, naming the caller's row input_row[r] when given, else r; on a refusal nothing of the store is written.
+    // Then they are narrowed (bf16, fp16) or quantised (q8) into the store.  An index without a store gets one of cap rows first.
+    // Returns once the rows are stored.
+    idb_status put_rows(uint64_t r0, uint64_t m, const uint32_t* input_row, const std::function<cudaError_t(float*)>& fill);
+    // m x dim host floats -> dst (m rows of nchunks * 4 floats on the device, zero padded), enqueued on the index's stream.
+    cudaError_t copy_rows_in(float* dst, const float* src, uint64_t m) const;
+    // Storage for at least `rows` points: rows, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
     // n rows.  Everything is allocated before anything is freed, so a failure leaves the index as it was.
     idb_status reserve_rows(uint64_t rows);
-    // Rows [r0, r0 + m) (r0 >= n, within cap) from m x dim host floats, as the build stores them: zero padded, normalised for a
-    // cosine index, narrowed for a bf16 / fp16 one, quantised for a q8 one; their zero rows INVALID; global_ids (m entries) into the
-    // id map when it exists.  fp16 / q8 rows beyond the storage's range are refused before anything of the index is written.
-    idb_status stage_rows(const float* rows, uint64_t r0, uint64_t m, const uint32_t* global_ids);
+    idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) widened to m x dim f32 on the host
+    // ----
+    // The zero rows of rows [r0, r0 + m) INVALID, and global_ids (m entries) into the id map when it exists (the insert, after put_rows).
+    idb_status stage_rows(uint64_t r0, uint64_t m, const uint32_t* global_ids);
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
-    idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) as n x dim f32 on the host
     int search_grid() const;
     // The visited tier of a traversal with this ef, and its launch window.  Caller holds ctx->mu.
     idb_status select_visited_tier(uint32_t ef, VisTier& tier, LaunchWindow& win);
@@ -325,21 +348,6 @@ static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRow
               "RowType mirrors IDB_STORAGE_*");
 // The storage values an index accepts (3 is not one of them).
 inline bool storage_known(uint32_t s) { return s <= IDB_STORAGE_F16 || s == IDB_STORAGE_Q8; }
-// q8 storage (DESIGN §3c): IDB_ERR_INVALID_ARG when one of the m staged rows (nchunks * 4 f32 each, the first dim used, on the device)
-// has a NaN or infinite element, or its header or a dequantised element would overflow f32; the message names the row (input_row[r]
-// when given, else r + row0) and element.  IDB_OK otherwise.
-idb_status check_q8_rows(const float* d_rows, uint64_t m, uint32_t nchunks, uint32_t dim, const uint32_t* input_row, uint64_t row0,
-                         int num_sms, cudaStream_t st);
-// m checked rows (nchunks * 4 f32 each) -> their codes (nchunks * 4 bytes each, padding codes 0) and headers.  Enqueued on st.
-cudaError_t quantize_q8(const float* src, uint64_t m, uint32_t nchunks, uint32_t dim, uint8_t* codes, float2* hdr, int num_sms,
-                        cudaStream_t st);
-// fp16 storage: IDB_ERR_INVALID_ARG when an element of the m staged rows (nchunks * 4 f32 each, on the device) is finite and rounds to
-// +-infinity in fp16 (|x| >= 65520), naming the row (input_row[r] when given, else r + row0) and element; IDB_OK otherwise.
-idb_status check_f16_range(const float* d_rows, uint64_t m, uint32_t nchunks, const uint32_t* input_row, uint64_t row0, int num_sms,
-                           cudaStream_t st);
-// count elements f32 -> dst in `type` (kRowBF16 / kRowF16), round to nearest even; back to f32 exactly.  Enqueued on st.
-cudaError_t narrow_elems(const float* src, uint16_t* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st);
-cudaError_t widen_elems(const uint16_t* src, float* dst, size_t count, uint32_t type, int num_sms, cudaStream_t st);
 // normalize_rows_kernel: dst[r] (nchunks * 4 floats, zero padded) = the canonical normalisation of src[r] (src_stride floats per row,
 // dim used, any alignment), one warp per row.  dst may equal src when src_stride == nchunks * 4.
 cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,

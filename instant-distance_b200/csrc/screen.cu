@@ -19,12 +19,6 @@ namespace idb {
 
 namespace {
 
-// Element i of the stored rows, widened exactly (row_type: RowType).
-__device__ __forceinline__ float stored_at(const void* pts, uint32_t row_type, size_t i) {
-    if (row_type == kRowF32) return reinterpret_cast<const float*>(pts)[i];
-    const uint32_t h = reinterpret_cast<const uint16_t*>(pts)[i];
-    return row_type == kRowBF16 ? __uint_as_float(h << 16) : widen_f16x2(h).x;
-}
 // order-preserving u32 image of a float (for atomicMin / atomicMax)
 __device__ __forceinline__ uint32_t ord_of(float f) {
     const uint32_t b = __float_as_uint(f);
@@ -33,15 +27,14 @@ __device__ __forceinline__ uint32_t ord_of(float f) {
 __device__ __forceinline__ float float_of_ord(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u); }
 
 // Blocks own ranges of rows, threads own elements: every step of a thread's loop is one coalesced slice of a row.
-__global__ void code_range_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint64_t rows_per_block, uint32_t* mn,
-                                  uint32_t* mx, uint32_t* bad) {
+__global__ void code_range_kernel(const StoredRows s, uint64_t n, uint64_t rows_per_block, uint32_t* mn, uint32_t* mx, uint32_t* bad) {
     const uint64_t r0 = (uint64_t)blockIdx.x * rows_per_block, r1 = min(n, r0 + rows_per_block);
     if (r0 >= r1) return;
-    for (uint32_t e = threadIdx.x; e < stride; e += blockDim.x) {
+    for (uint32_t e = threadIdx.x; e < s.stride; e += blockDim.x) {
         float lo = INFINITY, hi = -INFINITY;
         bool nonfinite = false;
         for (uint64_t r = r0; r < r1; ++r) {
-            const float x = stored_at(pts, row_type, r * stride + e);
+            const float x = stored_elem(s, r, e);
             nonfinite |= !isfinite(x);
             lo = fminf(lo, x);
             hi = fmaxf(hi, x);
@@ -70,8 +63,9 @@ __device__ __forceinline__ float code_of_value(float x, float offset, float step
 }
 
 // codes: rows of cstride bytes (4 code_words(nchunks)); the bytes past stride are zeroed beforehand.
-__global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t stride, uint32_t cstride, uint64_t rows_per_block,
-                                   float* prm, const uint32_t* step, unsigned char* codes) {
+__global__ void code_encode_kernel(const StoredRows s, uint64_t n, uint32_t cstride, uint64_t rows_per_block, float* prm, const uint32_t* step,
+                                   unsigned char* codes) {
+    const uint32_t stride = s.stride;
     const float S = __uint_as_float(*step);
     if (blockIdx.x == 0)
         for (uint32_t e = threadIdx.x; e < stride; e += blockDim.x) prm[e] = S;
@@ -81,7 +75,7 @@ __global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t 
         const float offset = prm[stride + e];
         float err = 0.f;
         for (uint64_t r = r0; r < r1; ++r) {
-            const float x = stored_at(pts, row_type, r * stride + e);
+            const float x = stored_elem(s, r, e);
             const float c = code_of_value(x, offset, S);
             codes[r * cstride + e] = (unsigned char)c;
             const float xt = __fmaf_rn(c, S, offset);  // x~ of the per-element float bound
@@ -93,10 +87,10 @@ __global__ void code_encode_kernel(const void* pts, uint32_t row_type, uint64_t 
 
 // One warp per row (grid-stride): r_x = ||x - x~||, rounded up, with x~_i = offset_i + c_i * S in real arithmetic, which lies in
 // [fmaf_rd(c, S, offset), fmaf_ru(c, S, offset)], so |x_i - x~_i| <= max(x_i - lo, hi - x_i).  err_max = max over the rows.
-__global__ void code_row_err_kernel(const void* pts, uint32_t row_type, uint64_t n, uint32_t nchunks, const float* prm,
-                                    const uint32_t* step, const uint32_t* codes, uint32_t* err_max) {
+__global__ void code_row_err_kernel(const StoredRows s, uint64_t n, const float* prm, const uint32_t* step, const uint32_t* codes,
+                                    uint32_t* err_max) {
     const float S = __uint_as_float(*step);
-    const uint32_t stride = nchunks * 4, cwords = code_words(nchunks);
+    const uint32_t stride = s.stride, nchunks = stride / 4, cwords = code_words(nchunks);
     const int lane = threadIdx.x & 31;
     const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
     float worst = 0.f;
@@ -107,7 +101,7 @@ __global__ void code_row_err_kernel(const void* pts, uint32_t row_type, uint64_t
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const uint32_t e = 4 * c + k;
-                const float x = stored_at(pts, row_type, r * stride + e), off = prm[stride + e], code = (float)((w >> (8 * k)) & 0xFFu);
+                const float x = stored_elem(s, r, e), off = prm[stride + e], code = (float)((w >> (8 * k)) & 0xFFu);
                 const float d = fmaxf(__fsub_ru(x, __fmaf_rd(code, S, off)), __fsub_ru(__fmaf_ru(code, S, off), x));
                 acc = __fmaf_ru(d, d, acc);
             }
@@ -169,7 +163,7 @@ idb_status Index::build_codes() {
     d_cparams = nullptr;
     if (!screen || n == 0 || row_type == kRowQ8) return IDB_OK;  // DESIGN §3c: q8 rows are one byte per element already
     const uint32_t stride = nchunks * 4, cstride = code_words(nchunks) * 4;
-    const void* pts = rows();
+    const StoredRows s = stored();
     const unsigned grid = (unsigned)std::min<uint64_t>((n + 63) / 64, (uint64_t)num_sms * 8);
     const uint64_t rows_per_block = (n + grid - 1) / grid;
     uint32_t* tmp = nullptr;  // [0, stride) min, [stride, 2 stride) max, [2 stride] non-finite flag, [2 stride + 1] S, [2 stride + 2] R
@@ -180,7 +174,7 @@ idb_status Index::build_codes() {
     if (e == cudaSuccess) e = fill_u32(tmp, stride, 0xFFFFFFFFu, stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(tmp + stride, 0, ((size_t)stride + 3) * 4, stream);
     if (e == cudaSuccess) {
-        code_range_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, rows_per_block, tmp, tmp + stride, tmp + 2 * stride);
+        code_range_kernel<<<grid, 128, 0, stream>>>(s, n, rows_per_block, tmp, tmp + stride, tmp + 2 * stride);
         e = cudaGetLastError();
     }
     uint32_t bad = 0;
@@ -191,9 +185,8 @@ idb_status Index::build_codes() {
         float* prm = reinterpret_cast<float*>(d_cparams);
         uint32_t* step = tmp + 2 * stride + 1;
         code_params_kernel<<<(stride + 127) / 128, 128, 0, stream>>>(tmp, tmp + stride, stride, prm, step);
-        code_encode_kernel<<<grid, 128, 0, stream>>>(pts, row_type, n, stride, cstride, rows_per_block, prm, step,
-                                                     reinterpret_cast<unsigned char*>(d_codes));
-        code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(pts, row_type, n, nchunks, prm, step, d_codes, step + 1);
+        code_encode_kernel<<<grid, 128, 0, stream>>>(s, n, cstride, rows_per_block, prm, step, reinterpret_cast<unsigned char*>(d_codes));
+        code_row_err_kernel<<<num_sms * 8, 256, 0, stream>>>(s, n, prm, step, d_codes, step + 1);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cudaMemcpyAsync(step_err, step, 8, cudaMemcpyDeviceToHost, stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
