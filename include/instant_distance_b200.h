@@ -63,7 +63,8 @@ typedef enum idb_status {
     IDB_ERR_NCCL = 4,
     IDB_ERR_IO = 5,
     IDB_ERR_FORMAT = 6,        /* malformed index file */
-    IDB_ERR_CAPACITY = 7,      /* an internal per-query structure overflowed even after the retry pass */
+    IDB_ERR_CAPACITY = 7,      /* an internal per-query structure overflowed even after the retry pass; or a range search
+                                  found more hits than its capacity */
     IDB_ERR_UNSUPPORTED = 8
 } idb_status;
 
@@ -209,6 +210,30 @@ IDB_API idb_status idb_exact_search_batch_f32(idb_index* index, const float* que
  * syncing (lane >= idb_index_num_lanes(): IDB_ERR_INVALID_ARG). */
 IDB_API idb_status idb_exact_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq,
                                                       uint32_t k, uint32_t* d_out_ids, float* d_out_dist, uint32_t* d_out_len);
+
+/* Exact range search (DESIGN.md §9b): every stored point within `radius` of each query.  Query q's hits are every PointId p whose
+ * reported distance (squared L2, or 1 - cos for a cosine index, as the exact search reports it) is <= radius, in the exact search's
+ * order (distance, then PointId; ids through the id map after ordering): a prefix of the query's full exact ordering.  A point at
+ * exactly `radius` is a hit (radius = 0 finds exact duplicates), a NaN distance never is, radius = +inf finds every point whose
+ * distance is not NaN, and a negative radius finds none.
+ * The output is CSR: query q's hits are out_ids[out_offsets[q] .. out_offsets[q + 1]) (out_offsets: nq + 1 entries,
+ * out_offsets[nq] = the total), with their distances at the same positions of out_dist (optional).  `capacity` is how many hits
+ * out_ids / out_dist hold, and the size of the call's device scratch (20 bytes per hit).  When the total exceeds it the call returns
+ * IDB_ERR_CAPACITY with out_offsets written and nothing else, so a caller can allocate exactly and call again; capacity = 0 is a
+ * counting call.  The rows are scanned once per call.  capacity <= 2^31 - 1 and nq < 2^31 - 1 (IDB_ERR_UNSUPPORTED beyond:
+ * the library's sort and scan take int sizes).  Takes an idle submission lane, like the exact search, and leaves the approximate-search
+ * diagnostics as they are.  Null index / queries or out_offsets (nq > 0) / out_ids (capacity > 0), or a NaN radius:
+ * IDB_ERR_INVALID_ARG.  nq == 0: IDB_OK, out_offsets[0] = 0 (when given). */
+IDB_API idb_status idb_range_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, float radius, uint64_t capacity,
+                                              uint64_t* out_offsets, uint32_t* out_ids, float* out_dist);
+/* Same, device pointers on the index's device (d_queries: nq x dim at any alignment; d_out_offsets 8-byte aligned), on submission
+ * lane `lane` (>= idb_index_num_lanes(): IDB_ERR_INVALID_ARG, even at nq = 0).  The total goes to the HOST word *out_total (null:
+ * IDB_ERR_INVALID_ARG), also with IDB_ERR_CAPACITY.  Unlike the other device entries this one returns only after the lane has run
+ * the call: the hits are ordered by a sort whose size is the total, which the host has to know first.  nq == 0: IDB_OK,
+ * *out_total = 0, nothing written on the device. */
+IDB_API idb_status idb_range_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq,
+                                                      float radius, uint64_t capacity, uint64_t* d_out_offsets,
+                                                      uint32_t* d_out_ids, float* d_out_dist, uint64_t* out_total);
 
 IDB_API uint32_t idb_index_num_lanes(void);
 IDB_API void* idb_index_lane_stream(idb_index* index, uint32_t lane);  /* cudaStream_t of that lane */

@@ -319,17 +319,15 @@ static bool host_ptr_is_pinned(const void* p) {
 // control blocks: a device-to-pageable cudaMemcpyAsync blocks inside the driver until the copy has run (i.e. until this call's K1 has
 // finished) and stalls the launches of other caller threads meanwhile — concurrent callers would never have a second batch queued
 // behind the running one.  Those results are staged in the lane's pinned buffer and copied out after the stream has been synchronised.
-idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len, Lane* const* ctrl_lanes,
-                     uint32_t n_ctrl) {
-    struct Part { void* user; const void* dev; size_t bytes; size_t off; };
-    Part parts[3] = {{out_ids, ln.ids, nq * k * 4, 0}, {out_dist, ln.dist, nq * k * 4, 0}, {out_len, ln.len, nq * 4, 0}};
+idb_status copy_to_host(Lane& ln, const HostCopy* parts, int n_parts, const std::function<cudaError_t()>& also) {
     bool staged = false;
     size_t total = 0;
-    for (Part& p : parts) {
-        if (!p.user) continue;
-        staged = staged || !host_ptr_is_pinned(p.user);
-        p.off = total;
-        total += (p.bytes + 63) / 64 * 64;
+    size_t off[4] = {};
+    for (int i = 0; i < n_parts; ++i) {
+        if (!parts[i].user) continue;
+        staged = staged || !host_ptr_is_pinned(parts[i].user);
+        off[i] = total;
+        total += (parts[i].bytes + 63) / 64 * 64;
     }
     if (staged && total > ln.h_out_cap) {
         if (ln.h_out) cudaFreeHost(ln.h_out);
@@ -338,15 +336,30 @@ idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float
         CUDA_TRY(cudaHostAlloc(reinterpret_cast<void**>(&ln.h_out), total + total / 4, cudaHostAllocDefault));
         ln.h_out_cap = total + total / 4;
     }
-    for (const Part& p : parts)
-        if (p.user)
-            CUDA_TRY(cudaMemcpyAsync(staged ? static_cast<void*>(ln.h_out + p.off) : p.user, p.dev, p.bytes, cudaMemcpyDeviceToHost, ln.stream));
-    for (uint32_t i = 0; i < n_ctrl; ++i)
-        if (ctrl_lanes[i]->last_nq)
-            CUDA_TRY(cudaMemcpyAsync(ctrl_lanes[i]->h_ctrl + 1, ctrl_lanes[i]->ctrl, sizeof(SearchCtrl), cudaMemcpyDeviceToHost, ln.stream));
+    for (int i = 0; i < n_parts; ++i)
+        if (parts[i].user)
+            CUDA_TRY(cudaMemcpyAsync(staged ? static_cast<void*>(ln.h_out + off[i]) : parts[i].user, parts[i].dev, parts[i].bytes,
+                                     cudaMemcpyDeviceToHost, ln.stream));
+    if (also) CUDA_TRY(also());
     CUDA_TRY(cudaStreamSynchronize(ln.stream));
-    for (const Part& p : parts)
-        if (staged && p.user) std::memcpy(p.user, ln.h_out + p.off, p.bytes);
+    for (int i = 0; i < n_parts; ++i)
+        if (staged && parts[i].user) std::memcpy(parts[i].user, ln.h_out + off[i], parts[i].bytes);
+    return IDB_OK;
+}
+
+idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len, Lane* const* ctrl_lanes,
+                     uint32_t n_ctrl) {
+    const HostCopy parts[3] = {{out_ids, ln.ids, nq * k * 4}, {out_dist, ln.dist, nq * k * 4}, {out_len, ln.len, nq * 4}};
+    const idb_status st = copy_to_host(ln, parts, 3, [&]() {
+        for (uint32_t i = 0; i < n_ctrl; ++i)
+            if (ctrl_lanes[i]->last_nq) {
+                const cudaError_t e = cudaMemcpyAsync(ctrl_lanes[i]->h_ctrl + 1, ctrl_lanes[i]->ctrl, sizeof(SearchCtrl),
+                                                      cudaMemcpyDeviceToHost, ln.stream);
+                if (e != cudaSuccess) return e;
+            }
+        return cudaSuccess;
+    });
+    if (st != IDB_OK) return st;
     uint64_t failed = 0;  // failures that survived the retry pass
     for (uint32_t i = 0; i < n_ctrl; ++i)
         if (ctrl_lanes[i]->last_nq) failed += ctrl_lanes[i]->h_ctrl[1].retry.fail_count;
@@ -367,11 +380,22 @@ idb_status require_device(int* count) {
 }
 
 idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shards, const void* comm, const uint32_t* lane,
-                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k) {
+                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k, const RangeCheck* rc) {
     if (f == Family::sharded && !comm) return fail(IDB_ERR_INVALID_ARG, "comm is null");
     if (f != Family::sharded && !shards[0]) return fail(IDB_ERR_INVALID_ARG, "index is null");
-    if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
-    if ((nq > 0 || f == Family::exact) && k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
+    if (f == Family::range) {
+        if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_offsets is null");
+        if (rc->capacity > 0 && !rc->ids)
+            return fail(IDB_ERR_INVALID_ARG, "out_ids is null with capacity %llu", (unsigned long long)rc->capacity);
+        if (std::isnan(rc->radius)) return fail(IDB_ERR_INVALID_ARG, "radius is NaN");
+        if (rc->device && !rc->out_total) return fail(IDB_ERR_INVALID_ARG, "out_total is null");
+        if (rc->capacity > kRangeMaxCapacity || nq >= kRangeMaxCapacity)
+            return fail(IDB_ERR_UNSUPPORTED, "the range search takes a capacity of at most %llu and fewer queries (capacity %llu, nq %llu)",
+                        (unsigned long long)kRangeMaxCapacity, (unsigned long long)rc->capacity, (unsigned long long)nq);
+    } else {
+        if (nq > 0 && (!queries || !out_ids)) return fail(IDB_ERR_INVALID_ARG, "queries/out_ids is null");
+        if ((nq > 0 || f == Family::exact) && k == 0) return fail(IDB_ERR_INVALID_ARG, "k must be >= 1");
+    }
     if (f == Family::exact && k > kExactMaxK)
         return fail(IDB_ERR_UNSUPPORTED, "k = %u > %u is not supported by the exact search", k, kExactMaxK);
     if (lane && *lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range (0..%d)", *lane, kLanes - 1);
@@ -388,6 +412,7 @@ void Lane::free_all() {
     cudaFree(ctrl); cudaFree(status); cudaFree(fail_list); cudaFree(counters);
     cudaFree(q); cudaFree(qn); cudaFree(ids); cudaFree(dist); cudaFree(len);
     cudaFree(keys_local); cudaFree(keys_all); cudaFree(shard_ids); cudaFree(exact_keys);
+    cudaFree(range_keys); cudaFree(range_qids); cudaFree(range_seg); cudaFree(range_off); cudaFree(range_tmp);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (ev_ctrl) cudaEventDestroy(ev_ctrl);

@@ -2,30 +2,20 @@
 // stored rows (DESIGN.md §9a).
 //
 // A warp holds QW queries in registers (lane l owns chunks l, l+32, ... of each, as in K1) and streams the rows of one slice of the
-// index NB at a time; every distance comes from lane_partial + batch_butterfly, the helpers K1 computes its distances with, so the
-// two agree bit for bit.  Each (query, slice) keeps a sorted list of its k smallest keys in global scratch; a new key is compared with
-// the list's k-th key and almost always rejected there.  Slices split the rows when the queries alone do not fill the device; their
+// index NB at a time (scan_step, scan.cuh), with K1's own distance bits.  Each (query, slice) keeps a sorted list of its k smallest
+// keys in global scratch; a new key is compared with the list's k-th key and almost always rejected there.  Slices split the rows when the queries alone do not fill the device; their
 // lists are merged by K4 (merge.cu).
 #include <algorithm>
 #include <cstring>
 
-#include "internal.cuh"
+#include "scan.cuh"
 
 namespace idb {
 
 namespace {
 
-constexpr int kExactWarps = 8;                 // warps per CTA: they walk the same rows in the same order (L1 serves the others)
 constexpr uint64_t kExactScratchKeys = 1ull << 25;  // keys of per-call list scratch (256 MB): larger batches run in query chunks
 constexpr uint32_t kExactMaxSliceKeys = 2048;  // slices x k: K4's cost grows with its square
-constexpr uint64_t kExactMinSliceRows = 1024;
-
-// Queries per warp (QW) and rows per step (NB) of each CH: about 32 registers of query and 32-64 of rows per lane.
-template <int CH>
-struct ExactShape {
-    static constexpr int QW = CH == 1 ? 8 : CH == 2 ? 4 : (CH == 3 || CH == 4 || CH == 6) ? 2 : 1;
-    static constexpr int NB = CH == 0 ? kLongRowsInFlight : CH == 1 ? 8 : CH <= 3 ? 4 : 2;
-};
 
 struct ExactArgs {
     GraphView g;
@@ -77,8 +67,8 @@ __device__ __forceinline__ uint64_t list_insert(uint64_t* L, uint32_t& cnt, uint
 }
 
 template <int CH, class RT>
-__global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs a) {
-    constexpr int QW = ExactShape<CH>::QW, NB = ExactShape<CH>::NB;
+__global__ void __launch_bounds__(kScanWarps * 32) exact_scan_kernel(ExactArgs a) {
+    constexpr int QW = ScanShape<CH>::QW;
     static_assert(CH > 0 || QW == 1, "long rows: one query per warp (it lives in shared memory)");
     extern __shared__ float4 sm_exact_q[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpc = blockDim.x >> 5;
@@ -104,6 +94,7 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
         q_from_f32<CH>(q[j], a.queries + qi * nchunks, nchunks, lane);
     }
 
+    constexpr int NB = ScanShape<CH>::NB;
     const uint32_t row_bytes = nchunks * RT::kChunkBytes;
     const char* lane_base = a.g.points + lane * RT::kChunkBytes;
     const bool mine_lane = lane < NB;
@@ -111,50 +102,7 @@ __global__ void __launch_bounds__(kExactWarps * 32) exact_scan_kernel(ExactArgs 
     for (uint64_t b0 = r0; b0 < r1; b0 += NB) {
         const uint32_t nb = r1 - b0 < (uint64_t)NB ? (uint32_t)(r1 - b0) : (uint32_t)NB;
         float d[QW];
-        if constexpr (CH == 0) {  // batch_distances_long's order: four chains per row carried across groups of 32 chunks
-            const char* row[NB];
-            typename RT::Hdr h[NB];
-            float4 acc[NB];
-#pragma unroll
-            for (int i = 0; i < NB; ++i) {
-                row[i] = lane_base + (size_t)(b0 + ((uint32_t)i < nb ? i : 0)) * row_bytes;
-                h[i] = RT::hdr(a.g, (uint32_t)(b0 + ((uint32_t)i < nb ? i : 0)));
-                acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-#pragma unroll 1
-            for (uint32_t j = 0; j < q[0].ngroups; ++j) {
-                const bool ok = lane + 32u * j < nchunks;
-                const float4 qq = q[0].s[lane + 32u * j];
-                typename RT::Raw v[NB];
-#pragma unroll
-                for (int i = 0; i < NB; ++i) v[i] = (ok && (uint32_t)i < nb) ? RT::ld_raw(row[i] + (size_t)j * 32 * RT::kChunkBytes) : RT::zero();
-#pragma unroll
-                for (int i = 0; i < NB; ++i) l2_step(acc[i], qq, widen_chunk<RT>(a.g, v[i], h[i], lane + 32u * j));
-            }
-            float p[NB];
-#pragma unroll
-            for (int i = 0; i < NB; ++i) p[i] = lane_sum(acc[i]);
-            d[0] = batch_butterfly<NB>(p, lane);
-        } else {  // batch_distances_impl's order, the rows shared by the warp's QW queries
-            typename RT::Raw v[NB][CH];
-            typename RT::Hdr h[NB];
-#pragma unroll
-            for (int i = 0; i < NB; ++i) {
-                const bool ok = (uint32_t)i < nb;
-                const char* row = lane_base + (size_t)(b0 + (ok ? i : 0)) * row_bytes;
-                h[i] = RT::hdr(a.g, (uint32_t)(b0 + (ok ? i : 0)));
-#pragma unroll
-                for (int j = 0; j < CH; ++j)
-                    v[i][j] = (ok && (uint32_t)(lane + 32 * j) < nchunks) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
-            }
-#pragma unroll
-            for (int qj = 0; qj < QW; ++qj) {
-                float p[NB];
-#pragma unroll
-                for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(a.g, q[qj].r, v[i], h[i], lane);
-                d[qj] = batch_butterfly<NB>(p, lane);  // lane l: row b0 + (l & (NB - 1))
-            }
-        }
+        scan_step<CH, RT>(a.g, nchunks, q, lane_base, row_bytes, b0, nb, lane, d);
         const uint32_t pid = (uint32_t)(b0 + (lane & (NB - 1)));
         const bool mine = mine_lane && (uint32_t)lane < nb;
 #pragma unroll
@@ -196,7 +144,7 @@ struct ScanChoice {
 };
 template <int CH>
 ScanChoice scan_choice(uint32_t row_type) {
-    return with_row_type(row_type, [](auto rt) { return ScanChoice{exact_scan_kernel<CH, decltype(rt)>, ExactShape<CH>::QW}; });
+    return with_row_type(row_type, [](auto rt) { return ScanChoice{exact_scan_kernel<CH, decltype(rt)>, ScanShape<CH>::QW}; });
 }
 ScanChoice pick_scan(uint32_t nchunks, uint32_t row_type) {
     switch (kernel_ch(nchunks)) {
@@ -230,30 +178,22 @@ static idb_status enqueue_exact(Index* ix, Lane& ln, const float* queries, bool 
     if (s != IDB_OK) return s;
 
     const ScanChoice sc = pick_scan(nchunks, ix->row_type);
-    int wpc = kExactWarps;
-    size_t smem = 0;
-    if (kernel_ch(nchunks) == 0) {  // one query per warp in shared memory: fewer warps per CTA for very long rows
-        int max_smem = 0;
-        CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ix->device));
-        const size_t per_warp = (size_t)(nchunks + 31) / 32 * 32 * 16;
-        wpc = (int)std::min<size_t>(kExactWarps, (size_t)max_smem / per_warp);
-        if (wpc < 1) return fail(IDB_ERR_UNSUPPORTED, "dim %u: one query does not fit the device's shared memory", ix->dim);
-        smem = per_warp * wpc;
-        if (smem > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(sc.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
-    int occ = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sc.fn, wpc * 32, smem));
+    ScanLaunch sl;
+    s = scan_launch(ix, sc.fn, &sl);
+    if (s != IDB_OK) return s;
+    const int wpc = sl.wpc, occ = sl.occ;
+    const size_t smem = sl.smem;
     const uint64_t q_per_cta = (uint64_t)wpc * sc.qw;
 
     // Slices: enough CTAs for about four waves of the device; K4 merges S lists of k keys per query, so S x k stays small, and a
-    // slice keeps at least kExactMinSliceRows rows.  S = 1 (no merge) when the queries alone fill the device.
+    // slice keeps at least kScanMinSliceRows rows.  S = 1 (no merge) when the queries alone fill the device.
     const uint64_t cap_keys = ix->exact_scratch_keys ? ix->exact_scratch_keys : kExactScratchKeys;
     const uint64_t nq_eff = std::max<uint64_t>(1, std::min<uint64_t>(nq, cap_keys / k));
     const uint64_t want_ctas = 4ull * std::max(1, occ) * ix->num_sms;
     const uint64_t q_ctas = (nq_eff + q_per_cta - 1) / q_per_cta;
     uint64_t S = (want_ctas + q_ctas - 1) / q_ctas;
     S = std::min<uint64_t>(S, std::max<uint64_t>(1, kExactMaxSliceKeys / k));
-    S = std::min<uint64_t>(S, (ix->n + kExactMinSliceRows - 1) / kExactMinSliceRows);
+    S = std::min<uint64_t>(S, (ix->n + kScanMinSliceRows - 1) / kScanMinSliceRows);
     S = std::max<uint64_t>(S, 1);
     int max_smem = 0;
     if (S > 1) {

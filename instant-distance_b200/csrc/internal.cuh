@@ -175,6 +175,13 @@ struct Lane {
     uint32_t* shard_ids = nullptr;  size_t shard_ids_cap = 0;   // the shard's K1 ids (its keys carry the results)
     // exact search: the (query, slice) k-lists of the current query chunk (exact.cu)
     uint64_t* exact_keys = nullptr; size_t exact_keys_cap = 0;
+    // range search (range.cu): the appended (key, query) pairs, the keys gathered into their queries' segments, the host call's
+    // offsets and the append counter, and CUB's scratch (in u64 words)
+    uint64_t* range_keys = nullptr; size_t range_keys_cap = 0;
+    uint32_t* range_qids = nullptr; size_t range_qids_cap = 0;
+    uint64_t* range_seg = nullptr;  size_t range_seg_cap = 0;
+    uint64_t* range_off = nullptr;  size_t range_off_cap = 0;
+    uint64_t* range_tmp = nullptr;  size_t range_tmp_cap = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // host API: results land here first when the caller's output buffers are pageable (see read_back in api.cu)
     unsigned char* h_out = nullptr; size_t h_out_cap = 0;   // pinned
@@ -325,9 +332,18 @@ idb_status require_device(int* count = nullptr);
 // nq = 0 and caps k at kExactMaxK; `lane` (optional) must name a lane, even when nq = 0; `sharded` checks comm before anything else
 // and the list of n_shards handles only when nq > 0 (the others check their one handle first).  nq = 0 passes once the checks that
 // apply to it have, without the device check: there is nothing to do.
-enum class Family { approx, exact, sharded };
+// `range` takes no k; out_ids stands for its offsets, and `rc` carries what else it checks.
+enum class Family { approx, exact, sharded, range };
+struct RangeCheck {
+    float radius;
+    uint64_t capacity;
+    const void* ids;
+    bool device;                 // the device entry, which reports the total in *out_total
+    const uint64_t* out_total;
+};
+constexpr uint64_t kRangeMaxCapacity = 0x7fffffffu;  // CUB's sorts and scans take int sizes: capacity <= this, nq + 1 <= this
 idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shards, const void* comm, const uint32_t* lane,
-                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k);
+                             const void* queries, uint64_t nq, const void* out_ids, uint32_t k, const RangeCheck* rc = nullptr);
 
 // Empty result lists on the stream: ids INVALID, distances +inf, lengths 0, keys kKeyNone (each output optional but ids).
 cudaError_t write_empty(cudaStream_t st, uint64_t nq, uint32_t k, uint32_t* ids, float* dist, uint32_t* len, uint64_t* keys);
@@ -342,6 +358,14 @@ idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged
 // stream, and fails with IDB_ERR_CAPACITY when queries overflowed even the retry pass of those calls.
 idb_status read_back(Lane& ln, uint64_t nq, uint32_t k, uint32_t* out_ids, float* out_dist, uint32_t* out_len, Lane* const* ctrl_lanes,
                      uint32_t n_ctrl);
+// Device-to-host copies on ln.stream (at most 4), each into the caller's buffer `user` (skipped when null), staged through the
+// lane's pinned buffer when any of them is pageable; `also` enqueues more work behind them.  Then synchronises the stream.
+struct HostCopy {
+    void* user;
+    const void* dev;
+    size_t bytes;
+};
+idb_status copy_to_host(Lane& ln, const HostCopy* parts, int n_parts, const std::function<cudaError_t()>& also = nullptr);
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
 static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16 && kRowQ8 == IDB_STORAGE_Q8,

@@ -8,6 +8,8 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
   * `Hnsw.search_many / HnswMap.search_many` expose the batched search the GPU is built for;
   * `Hnsw.search_exact / HnswMap.search_exact` return the exact k nearest points (a scan of every point, ties by lower PointId),
     the ground truth to tune `ef_search` against;
+  * `Hnsw.search_range / HnswMap.search_range` return every point within a radius of each query (exact, however many there are;
+    DESIGN.md §9b), nearest first, as CSR;
   * `Hnsw.insert / HnswMap.insert` append points to a built or loaded index (layer 0 only, PointIds continue from the current
     count; DESIGN.md §6);
   * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
@@ -135,6 +137,12 @@ class Hnsw:
         """Exact k-NN over every point of the index: returns (ids [nq, k], distances [nq, k], lens [nq]) like search_many."""
         q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
         return self._ix.exact_search(q, k=k)
+
+    def search_range(self, points, radius):
+        """Every point within `radius` of each query (distance <= radius, in the index's metric), exact: returns (offsets [nq + 1],
+        ids [total], distances [total]); query i's neighbours are ids[offsets[i]:offsets[i + 1]], nearest first, ties by PointId."""
+        q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
+        return self._ix.range_search(q, radius)
 
     def _insert(self, points, config, on_partial=None):
         """on_partial(k): called before an IdbError propagates, with how many of the points the index kept (an insert that fails

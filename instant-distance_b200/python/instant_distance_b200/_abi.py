@@ -12,6 +12,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 LIB_PATH = os.environ.get("IDB_LIB_PATH") or os.path.join(_PKG, "lib", "libinstant_distance_b200.so")  # (IDB_LIB_PATH: A/B builds)
 
 INVALID = 0xFFFFFFFF
+RANGE_MAX_CAPACITY = 0x7FFFFFFF  # the range search's largest capacity (and nq)
 
 OK, ERR_INVALID_ARG, ERR_OOM, ERR_CUDA, ERR_NCCL, ERR_IO, ERR_FORMAT, ERR_CAPACITY, ERR_UNSUPPORTED = range(9)
 
@@ -26,6 +27,7 @@ SYMBOLS = [
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
     "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32", "idb_index_load_storage",
+    "idb_range_search_batch_f32", "idb_range_search_batch_device_lane",
 ]
 
 
@@ -82,6 +84,8 @@ def lib():
     L.idb_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, vp]
     L.idb_exact_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, u32p, f32p, u32p]
     L.idb_exact_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, vp, vp, vp]
+    L.idb_range_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_float, C.c_uint64, u64p, u32p, f32p]
+    L.idb_range_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_float, C.c_uint64, vp, vp, vp, u64p]
     L.idb_last_search_counters.argtypes = [vp, C.c_uint64, u64p]
     L.idb_last_search_failures.argtypes = [vp, C.c_uint32, u32p]
     L.idb_last_search_retried.argtypes = [vp, C.c_uint32, u32p]
@@ -310,6 +314,38 @@ class Index:
     def exact_search_device(self, d_queries, nq, k, d_ids, d_dist, d_len, lane=0):
         """Asynchronous exact k-NN on device buffers, enqueued on submission lane `lane`."""
         check(lib().idb_exact_search_batch_device_lane(self._h, lane, d_queries, nq, k, d_ids, d_dist, d_len))
+
+    def range_search(self, queries, radius, capacity=None):
+        """Exact range search (idb_range_search_batch_f32): every point within `radius` of each query, as CSR (offsets u64 [nq + 1],
+        ids u32 [total], dist f32 [total]); query i's hits are ids[offsets[i]:offsets[i + 1]], nearest first.  capacity=None: a first
+        guess, and once more with the exact total when the hits did not fit."""
+        q = self._queries(queries)
+        nq = q.shape[0]
+        guess = capacity is None
+        cap = min(max(64 * nq, 1 << 16), RANGE_MAX_CAPACITY) if guess else int(capacity)
+        offsets = np.empty(nq + 1, dtype=np.uint64)
+        while True:
+            ids = np.empty(cap, dtype=np.uint32)
+            dist = np.empty(cap, dtype=np.float32)
+            st = lib().idb_range_search_batch_f32(self._h, ptr(q, C.c_float), nq, float(radius), cap, ptr(offsets, C.c_uint64),
+                                                  ptr(ids, C.c_uint32), ptr(dist, C.c_float))
+            if st == ERR_CAPACITY and guess:
+                guess, cap = False, int(offsets[-1])
+                continue
+            check(st)
+            total = int(offsets[-1])
+            return offsets, ids[:total].copy(), dist[:total].copy()
+
+    def range_search_device(self, d_queries, nq, radius, capacity, d_offsets, d_ids, d_dist, lane=0):
+        """Exact range search on device buffers on submission lane `lane`; returns the total (raises IdbError with status
+        ERR_CAPACITY, the offsets written, when it exceeds `capacity`).  Returns once the lane has run the call."""
+        total = C.c_uint64()
+        st = lib().idb_range_search_batch_device_lane(self._h, lane, d_queries, nq, float(radius), capacity, d_offsets, d_ids, d_dist,
+                                                       C.byref(total))
+        if st == ERR_CAPACITY:
+            raise IdbError(st, lib().idb_last_error().decode("utf-8", "replace") + f" (total {int(total.value)})")
+        check(st)
+        return int(total.value)
 
     def lane_stream(self, lane):
         return lib().idb_index_lane_stream(self._h, lane)
