@@ -138,6 +138,30 @@ IDB_API idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, con
 IDB_API idb_status idb_index_insert_f32(idb_index* index, const float* rows, uint64_t m, uint32_t dim, const idb_params* params,
                                         const uint32_t* global_ids, uint32_t* out_ids);
 
+/* Remove: take the m points pids[0..m) out of an index of n points (DESIGN.md §6b).
+ *   - Repair: on every layer, each surviving row that lists a removed id is selected again.  Its candidates are its own entries
+ *     and the entries of the row of each removed id it lists (one hop: removed ids in those rows are dropped, not followed), without
+ *     the point itself and without removed ids.  The ef_construction nearest of them, by (distance, PointId), go through
+ *     select_heuristic (core:636-698) with keep_pruned and the 2M cap, or in simple mode the first 2M are taken; an upper row keeps
+ *     the first M (UpperNode::from_zero, types:65-71).  A row that lists no removed id is not touched.  An entry is any value other
+ *     than INVALID.
+ *   - Compaction, in order: new(x) = x - |{r in pids : r < x}|.  Every entry, the rows, the id map and the layer sizes follow:
+ *     n' = n - m, n_l' = |[0, n_l) minus pids|, and the upper layers left with no point are dropped.  Layer l still holds
+ *     [0, n_l'), and the entry point is the lowest surviving PointId.  out_new_ids (n entries, may be NULL) receives new(x), or
+ *     INVALID for a removed point.
+ *   - params: ef_construction (1..1024), heuristic and keep_pruned are read; M must equal the index's M; extend_candidates is
+ *     refused as by the build; everything else is ignored.  A pid >= n or a repeated pid is IDB_ERR_INVALID_ARG, naming its position
+ *     in pids.  m = 0 does nothing; m = n leaves an empty index of the same dim, storage and metric, which a later insert fills as
+ *     it fills any empty index.
+ *   - Exclusive (&mut self): searches on other threads wait until the removal has finished and see the index before or after it.
+ *   - Failures: an argument error or a failed allocation leaves the index as it was (every buffer, the compacted storage included,
+ *     is allocated before the first row is written, so the call needs room for a second copy of the index while it runs).
+ *   - Known limits: a surviving point whose only in-links came from removed points can become unreachable; a row whose candidates
+ *     were all removed ends up empty; the upper layers are not refilled from below.  The screening table is rebuilt from the rows
+ *     that remain. */
+IDB_API idb_status idb_index_remove(idb_index* index, const uint32_t* pids, uint64_t m, const idb_params* params,
+                                    uint32_t* out_new_ids);
+
 /* "Search a given graph": adopt a graph built elsewhere (the reference, the oracle, a loaded .idx file).
  * This is the parity entry point.  Mirrors the fields of `Hnsw` (core:194-199):
  *   points   n x dim, PointId order                       (Hnsw::points)

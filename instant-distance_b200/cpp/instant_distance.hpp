@@ -162,6 +162,34 @@ class Hnsw {
         for (Point& pt : points) points_.push_back(std::move(pt));
         return out;
     }
+    // Not in the reference: removes the points `pids` (distinct PointIds, idb_index_remove).  The rows that listed a removed point
+    // are selected again with ef_construction and the heuristic (nullopt: the simple selection); the other points keep their order
+    // and are renumbered without gaps, so points_ drops the removed ones.  Returns, for each point the index had, its PointId
+    // afterwards, or nullopt for a removed one.  Like a `&mut self` method it invalidates the Items of earlier searches.
+    std::vector<std::optional<PointId>> remove(const std::vector<PointId>& pids, size_t ef_construction = 100,
+                                               std::optional<Heuristic> heuristic = Heuristic{}) {
+        idb_info info;
+        check(idb_index_info(raw_, &info));
+        idb_params p;
+        check(idb_params_default(&p));
+        p.M = info.M;
+        p.ef_construction = (uint32_t)ef_construction;
+        p.heuristic = heuristic ? 1 : 0;
+        p.extend_candidates = heuristic && heuristic->extend_candidates;
+        p.keep_pruned = !heuristic || heuristic->keep_pruned;
+        std::vector<uint32_t> raw(pids.size()), new_ids(info.n);
+        for (size_t i = 0; i < pids.size(); ++i) raw[i] = pids[i].raw;
+        check(idb_index_remove(raw_, raw.data(), raw.size(), &p, new_ids.data()));
+        std::vector<std::optional<PointId>> out(info.n);
+        std::vector<Point> kept;
+        for (size_t x = 0; x < info.n; ++x) {
+            if (new_ids[x] == IDB_INVALID) continue;
+            out[x] = PointId{new_ids[x]};
+            kept.push_back(std::move(points_[x]));
+        }
+        points_ = std::move(kept);
+        return out;
+    }
     // lib.rs:386-391, types.rs:269-275
     const std::vector<Point>& iter() const { return points_; }
     const Point& operator[](PointId p) const { return points_.at(p.raw); }
@@ -196,6 +224,16 @@ class HnswMap {
             for (size_t i = 0; i < hnsw_.iter().size() - n0; ++i) values.push_back(std::move(vals[i]));
             throw;
         }
+    }
+    // Hnsw::remove; the values of the removed points are dropped, the others follow their points' new PointIds.
+    std::vector<std::optional<PointId>> remove(const std::vector<PointId>& pids, size_t ef_construction = 100,
+                                               std::optional<Heuristic> heuristic = Heuristic{}) {
+        std::vector<std::optional<PointId>> new_ids = hnsw_.remove(pids, ef_construction, heuristic);
+        std::vector<V> kept;
+        for (size_t x = 0; x < new_ids.size(); ++x)
+            if (new_ids[x]) kept.push_back(std::move(values[x]));
+        values = std::move(kept);
+        return new_ids;
     }
 };
 

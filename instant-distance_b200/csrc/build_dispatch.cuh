@@ -64,4 +64,23 @@ cudaError_t build_dispatch(const BuildArgs& a, const BuildLaunch& l, cudaStream_
     return with_row_type(a.g.row_type, [&](auto rt) { return build_dispatch_rt<CH, B, NB, decltype(rt)>(a, l, st); });
 }
 
+// K2's ladder, for other kernels built on select_heuristic_warp (remove.cu): f(CH, NB) as integral constants, with the (CH, NB) that
+// build_chN.cu instantiates for rows of `nchunks` chunks.
+template <int CH_, int NB_>
+struct K2Cell {
+    static constexpr int CH = CH_, NB = NB_;
+};
+template <class F>
+cudaError_t with_k2_cell(uint32_t nchunks, F&& f) {
+    switch (kernel_ch(nchunks)) {
+        case 1: return f(K2Cell<1, 16>());
+        case 2: return f(K2Cell<2, 8>());
+        case 3: return f(K2Cell<3, 4>());
+        case 4: return f(K2Cell<4, 4>());
+        case 6: return f(K2Cell<6, 2>());
+        case 8: return f(K2Cell<8, 2>());
+        default: return f(K2Cell<0, kLongRowsInFlight>());
+    }
+}
+
 }  // namespace idb

@@ -295,6 +295,8 @@ struct Index {
     // Storage for at least `rows` points: rows, zero and the id map move to buffers of max(rows, 2 cap) rows holding the same first
     // n rows.  Everything is allocated before anything is freed, so a failure leaves the index as it was.
     idb_status reserve_rows(uint64_t rows);
+    size_t row_bytes() const;                                           // bytes of one stored row
+    cudaError_t alloc_rows(uint64_t rows, void** pts, float2** hdr) const;  // a store of `rows` rows (and q8 headers); frees nothing
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) widened to m x dim f32 on the host
     // ----
     // The zero rows of rows [r0, r0 + m) INVALID, and global_ids (m entries) into the id map when it exists (the insert, after put_rows).

@@ -204,6 +204,10 @@ idb_status Index::put_rows(uint64_t r0, uint64_t m, const uint32_t* input_row, c
     return s;
 }
 
+size_t Index::row_bytes() const { return (size_t)nchunks * 4 * elem_bytes(row_type); }
+
+cudaError_t Index::alloc_rows(uint64_t rows, void** pts, float2** hdr) const { return alloc_store(*this, rows, pts, hdr); }
+
 cudaError_t Index::copy_rows_in(float* dst, const float* src, uint64_t m) const {
     const size_t stride = (size_t)nchunks * 4;
     if (stride == dim) return cudaMemcpyAsync(dst, src, m * stride * 4, cudaMemcpyHostToDevice, stream);

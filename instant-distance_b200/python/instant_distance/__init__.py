@@ -144,17 +144,23 @@ class Hnsw:
         q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
         return self._ix.range_search(q, radius)
 
-    def _insert(self, points, config, on_partial=None):
-        """on_partial(k): called before an IdbError propagates, with how many of the points the index kept (an insert that fails
-        with ERR_CAPACITY keeps the batches before the failing one)."""
-        m = _to_matrix(points, self._dim)
-        config = Config() if config is None else config
+    @staticmethod
+    def _link_kw(config):
+        """The idb_params fields an insert or a removal reads from config: ef_construction and the heuristic."""
         kw = dict(ef_construction=config.ef_construction)
         if config.heuristic is None:
             kw["heuristic"] = 0
         else:
             kw.update(heuristic=1, extend_candidates=int(bool(config.heuristic.extend_candidates)),
                       keep_pruned=int(bool(config.heuristic.keep_pruned)))
+        return kw
+
+    def _insert(self, points, config, on_partial=None):
+        """on_partial(k): called before an IdbError propagates, with how many of the points the index kept (an insert that fails
+        with ERR_CAPACITY keeps the batches before the failing one)."""
+        m = _to_matrix(points, self._dim)
+        config = Config() if config is None else config
+        kw = self._link_kw(config)
         n0 = int(self._ix.info().n)
         try:
             return [int(i) for i in self._ix.insert(m, **kw)]
@@ -168,6 +174,14 @@ class Hnsw:
         Construction::insert on layer 0 (the upper layers keep sampling the points the index was built with).  config supplies
         ef_construction and the heuristic (None: Config() defaults); points are zero-padded to the index's dimension."""
         return self._insert(points, config)
+
+    def remove(self, pids, config=None):
+        """Not in the reference module: removes the points `pids` (distinct PointIds) and returns new_ids, one entry per point the
+        index had: the point's PointId afterwards, or INVALID (0xFFFFFFFF) for a removed one.  The surviving points keep their order
+        and are renumbered without gaps.  The rows that listed a removed point are re-selected from their own entries and the
+        removed point's neighbours; config supplies ef_construction and the heuristic (None: Config() defaults)."""
+        config = Config() if config is None else config
+        return [int(i) for i in self._ix.remove(pids, **self._link_kw(config))]
 
     def dump(self, fname):
         """py:131-137: bincode layout of `Hnsw` (ef_search, points, zero, layers)."""
@@ -208,6 +222,13 @@ class HnswMap(Hnsw):
         ids = self._insert(points, config, on_partial=lambda kept: self._values.extend(vals[:kept]))
         self._values.extend(vals)
         return ids
+
+    def remove(self, pids, config=None):
+        """Hnsw.remove; the values of the removed points are dropped and the others follow their points' new PointIds (so `dump`
+        writes them in PointId order)."""
+        new_ids = Hnsw.remove(self, pids, config)
+        self._values = [v for v, y in zip(self._values, new_ids) if y != _abi.INVALID]
+        return new_ids
 
     @property
     def values(self):

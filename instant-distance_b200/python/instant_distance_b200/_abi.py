@@ -27,7 +27,7 @@ SYMBOLS = [
     "idb_build_ex", "idb_index_from_graph_ex", "idb_index_load_ex", "idb_normalize_f32", "idb_index_metric",
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
     "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32", "idb_index_load_storage",
-    "idb_range_search_batch_f32", "idb_range_search_batch_device_lane",
+    "idb_range_search_batch_f32", "idb_range_search_batch_device_lane", "idb_index_remove",
 ]
 
 
@@ -77,6 +77,7 @@ def lib():
     L.idb_index_load_ex.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
     L.idb_index_load_storage.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int32, C.POINTER(vp), u64p]
     L.idb_index_insert_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.POINTER(Params), u32p, u32p]
+    L.idb_index_remove.argtypes = [vp, u32p, C.c_uint64, C.POINTER(Params), u32p]
     L.idb_normalize_f32.argtypes = [f32p, C.c_uint64, C.c_uint32, C.c_int32, f32p]
     L.idb_index_metric.argtypes = [vp, u32p]
     L.idb_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.c_uint32, u32p, f32p, u32p]
@@ -248,6 +249,18 @@ class Index:
         check(lib().idb_index_insert_f32(self._h, ptr(rows, C.c_float), m, dim, C.byref(p), None if g is None else ptr(g, C.c_uint32),
                                          ptr(ids, C.c_uint32)))
         return ids
+
+    def remove(self, pids, **kw):
+        """Removes the points `pids` (distinct PointIds) from the index (idb_index_remove); returns new_ids (n entries): the PointId
+        each point has afterwards, or INVALID for a removed one.  kw: idb_params fields (ef_construction, heuristic, keep_pruned;
+        M defaults to the index's)."""
+        pids = np.ascontiguousarray(pids, dtype=np.uint32).reshape(-1)
+        kw.setdefault("M", int(self.info().M))
+        p = default_params(**kw)
+        n = int(self.info().n)
+        new_ids = np.empty(max(n, 1), dtype=np.uint32)
+        check(lib().idb_index_remove(self._h, ptr(pids, C.c_uint32), pids.shape[0], C.byref(p), ptr(new_ids, C.c_uint32)))
+        return new_ids[:n]
 
     def save(self, path):
         check(lib().idb_index_save(self._h, os.fsencode(path)))

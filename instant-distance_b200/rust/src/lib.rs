@@ -43,6 +43,7 @@ extern "C" {
     fn idb_range_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32) -> i32;
     fn idb_range_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32, total: *mut u64) -> i32;
     fn idb_index_insert_f32(ix: *mut IdbIndex, rows: *const f32, m: u64, dim: u32, p: *const IdbParams, global_ids: *const u32, out_ids: *mut u32) -> i32;
+    fn idb_index_remove(ix: *mut IdbIndex, pids: *const u32, m: u64, p: *const IdbParams, out_new_ids: *mut u32) -> i32;
     fn idb_index_free(ix: *mut IdbIndex);
     fn idb_last_error() -> *const c_char;
     // Batched / device-side / multi-GPU entry points (no counterpart in the reference; see include/instant_distance_b200.h):
@@ -137,7 +138,7 @@ impl Builder {
         assert_eq!(rc, 0, "{}", last_error()); // the reference's build is infallible
         let mut shuffled = points.clone(); // Hnsw::points is in PointId order (lib.rs:263-270)
         for (orig, pid) in ids.iter().enumerate() { shuffled[*pid as usize] = points[orig].clone(); }
-        (Hnsw { raw, points: shuffled, ef_search: self.ef_search }, ids.into_iter().map(PointId).collect())
+        (Hnsw { raw, points: shuffled, ef_search: self.ef_search, m: p.m }, ids.into_iter().map(PointId).collect())
     }
     /// lib.rs:78-80 -> HnswMap::new (lib.rs:141-152)
     pub fn build<V: Clone>(self, points: Vec<F32Point>, values: Vec<V>) -> HnswMap<V> {
@@ -154,7 +155,7 @@ impl Builder {
 pub struct Search { nearest: Vec<(f32, PointId)> }
 
 /// lib.rs:193-199
-pub struct Hnsw { raw: *mut IdbIndex, points: Vec<F32Point>, ef_search: usize }
+pub struct Hnsw { raw: *mut IdbIndex, points: Vec<F32Point>, ef_search: usize, m: u32 }
 unsafe impl Send for Hnsw {}
 unsafe impl Sync for Hnsw {} // lib.rs:352-356: concurrent searches each take a submission lane inside the library and overlap on the device
 impl Drop for Hnsw {
@@ -198,6 +199,24 @@ impl Hnsw {
             return (0..offsets[1] as usize).map(|i| (dist[i], PointId(ids[i]))).collect();
         }
     }
+    /// Not in the reference: removes the points `pids` (distinct PointIds).  The rows that listed a removed point are selected again
+    /// with `ef_construction` and `heuristic` (None: the simple selection); the other points keep their order and are renumbered
+    /// without gaps.  Returns, for each point the index had, its PointId afterwards, or None for a removed one.
+    pub fn remove(&mut self, pids: &[PointId], ef_construction: usize, heuristic: Option<Heuristic>) -> Vec<Option<PointId>> {
+        let mut p = unsafe { std::mem::zeroed::<IdbParams>() };
+        unsafe { idb_params_default(&mut p) };
+        p.m = self.m;
+        p.ef_construction = ef_construction as u32;
+        p.heuristic = heuristic.is_some() as i32;
+        if let Some(h) = heuristic { p.extend_candidates = h.extend_candidates as i32; p.keep_pruned = h.keep_pruned as i32; }
+        let raw: Vec<u32> = pids.iter().map(|pid| pid.0).collect();
+        let mut new_ids = vec![u32::MAX; self.points.len()];
+        let rc = unsafe { idb_index_remove(self.raw, raw.as_ptr(), raw.len() as u64, &p, new_ids.as_mut_ptr()) };
+        assert_eq!(rc, 0, "{}", last_error());
+        let old = std::mem::take(&mut self.points);
+        self.points = old.into_iter().zip(&new_ids).filter(|(_, y)| **y != u32::MAX).map(|(pt, _)| pt).collect();
+        new_ids.into_iter().map(|y| if y == u32::MAX { None } else { Some(PointId(y)) }).collect()
+    }
     pub fn iter(&self) -> impl Iterator<Item = (PointId, &F32Point)> { self.points.iter().enumerate().map(|(i, p)| (PointId(i as u32), p)) }
 }
 impl std::ops::Index<PointId> for Hnsw {
@@ -213,4 +232,11 @@ impl<V: Clone> HnswMap<V> {
         self.hnsw.search(point, search).map(move |it| MapItem { distance: it.distance, pid: it.pid, point: it.point, value: &self.values[it.pid.0 as usize] })
     }
     pub fn iter(&self) -> impl Iterator<Item = (PointId, &F32Point)> { self.hnsw.iter() }
+    /// Hnsw::remove; the values of the removed points are dropped, the others follow their points' new PointIds.
+    pub fn remove(&mut self, pids: &[PointId], ef_construction: usize, heuristic: Option<Heuristic>) -> Vec<Option<PointId>> {
+        let new_ids = self.hnsw.remove(pids, ef_construction, heuristic);
+        let old = std::mem::take(&mut self.values);
+        self.values = old.into_iter().zip(&new_ids).filter(|(_, y)| y.is_some()).map(|(v, _)| v).collect();
+        new_ids
+    }
 }
