@@ -365,7 +365,8 @@ typedef struct idb_comm idb_comm;
 IDB_API idb_status idb_comm_unique_id(void* out_unique_id /* IDB_UNIQUE_ID_BYTES, made on one rank, shared by the host app */);
 IDB_API idb_status idb_comm_create(const void* unique_id, int32_t rank, int32_t world, int32_t device, idb_comm** out);
 IDB_API void idb_comm_free(idb_comm* comm);
-/* global_ids[pid] = the caller's id of the row that became PointId pid on this shard (NULL clears the map). */
+/* global_ids[pid] = the caller's id of the row that became PointId pid on this shard (NULL clears the map).
+ * Exclusive (&mut self): searches on other threads wait for it and see the map before or after it. */
 IDB_API idb_status idb_index_set_id_map(idb_index* index, const uint32_t* global_ids);
 /* Collective over `comm`: every rank passes the same queries.  out_ids are GLOBAL ids. */
 IDB_API idb_status idb_sharded_search_batch_f32(idb_index* shard, idb_comm* comm, const float* queries, uint64_t nq, uint32_t ef_search,

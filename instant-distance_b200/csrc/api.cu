@@ -1,7 +1,7 @@
 // api.cu — C ABI (include/instant_distance_b200.h) + the batched search kernel.
 //
-// Host side of the drop-in boundary: owns the row-major point matrix and the per-layer fixed-stride adjacency
-// ("CSR with implicit row_ptr = pid * stride", rows INVALID-terminated) in HBM, and launches the sm_90a kernels.
+// Host side of the drop-in boundary: the index object, whose row-major point matrix (rows.cu) and per-layer fixed-stride adjacency
+// ("CSR with implicit row_ptr = pid * stride", rows INVALID-terminated; graph.cu) live in HBM, and the sm_90a kernels' launches.
 // No PyTorch, no CPU fallback: if the CUDA runtime reports no device every compute entry point fails loudly.
 #include "internal.cuh"
 
@@ -76,41 +76,6 @@ cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, ui
     const uint64_t blocks = std::min<uint64_t>((n + 7) / 8, (uint64_t)num_sms * 16);
     normalize_rows_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, src_stride, reinterpret_cast<float4*>(dst), n, dim, nchunks);
     return cudaGetLastError();
-}
-
-// Adjacency sanity check for graphs adopted from outside (idb_index_from_graph_*, idb_index_load): every entry must be
-// INVALID or a PointId below `limit`; otherwise the traversal would read out of bounds.
-__global__ void validate_rows_kernel(const uint32_t* rows, size_t count, uint32_t limit, uint32_t* bad) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < count; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t v = rows[i];
-        if (v != kInvalid && v >= limit) atomicAdd(bad, 1u);
-    }
-}
-
-// Does any adjacency row list a PointId twice?  (The b16 visited flavour assumes it does not; graphs built by this library or by the
-// reference never do.)  One warp per row of `width` <= 128 entries.
-__global__ void repeated_ids_kernel(const uint32_t* rows, size_t n_rows, uint32_t width, uint32_t* repeats) {
-    const int lane = threadIdx.x & 31;
-    const size_t wpb = blockDim.x >> 5;
-    for (size_t r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n_rows; r += (size_t)gridDim.x * wpb) {
-        uint32_t e[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) e[t] = (uint32_t)(lane + 32 * t) < width ? rows[r * width + lane + 32 * t] : kInvalid;
-        bool rep = false;
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-            const uint32_t peers = __match_any_sync(kFullMask, e[t] == kInvalid ? (0x80000000u | (uint32_t)lane) + 0u : e[t]);
-            rep |= e[t] != kInvalid && (peers & ((1u << lane) - 1u));
-#pragma unroll
-            for (int t2 = 0; t2 < 4; ++t2)
-                if (t2 > t)
-                    for (int src = 0; src < 32; ++src) {
-                        const uint32_t o = __shfl_sync(kFullMask, e[t], src);
-                        rep |= o != kInvalid && o == e[t2];
-                    }
-        }
-        if (__any_sync(kFullMask, rep) && lane == 0) atomicAdd(repeats, 1u);
-    }
 }
 
 __global__ void nsmid_kernel(uint32_t* out) { asm volatile("mov.u32 %0, %%nsmid;" : "=r"(*out)); }
@@ -444,6 +409,19 @@ Lane& Index::pick_lane() {
     return ln;
 }
 
+ExclusiveIndex::ExclusiveIndex(Index* index) : ix(index) {
+    ix->mu.lock();
+    for (auto& ln : ix->lanes) ln.mu.lock();
+    drained = cudaSetDevice(ix->device);
+    for (auto& ln : ix->lanes)
+        if (drained == cudaSuccess) drained = cudaStreamSynchronize(ln.stream);
+}
+
+ExclusiveIndex::~ExclusiveIndex() {
+    for (auto& ln : ix->lanes) ln.mu.unlock();
+    ix->mu.unlock();
+}
+
 idb_status Index::last_search(uint32_t lane, bool latest, SearchCtrl* ctrl, uint32_t* kernel) {
     if (latest && lane == 0xFFFFFFFFu) lane = (uint32_t)last_lane.load();
     if (lane >= (uint32_t)kLanes) return fail(IDB_ERR_INVALID_ARG, "lane %u out of range", lane);
@@ -529,7 +507,7 @@ idb_status Index::select_visited_tier(uint32_t ef, VisTier& t, LaunchWindow& win
     }
     const uint32_t nb = std::min<uint32_t>((b16_bytes - kB16Stash * 4) / 32, 2040u);  // buckets over both segments
     const uint32_t nb_lo = std::min(nb, nb_lo_max);
-    const bool b16_exact = rows_distinct && (n + 32767) / 32768 <= nb;
+    const bool b16_exact = graph.rows_distinct && (n + 32767) / 32768 <= nb;
     int tier = vis_tier;
     if (tier == 2 && !b16_exact) tier = -1;
     if (tier < 0) tier = (b16_exact && level > 0) ? 2 : -1;
@@ -680,21 +658,14 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, 
     return IDB_OK;
 }
 
-idb_status Index::stage_rows(uint64_t r0, uint64_t m, const uint32_t* global_ids) {
-    CUDA_TRY(fill_u32(d_zero + r0 * 2 * M, m * 2 * M, kInvalid, stream));
-    if (d_id_map) CUDA_TRY(cudaMemcpyAsync(d_id_map + r0, global_ids, m * 4, cudaMemcpyHostToDevice, stream));
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    return IDB_OK;
-}
-
 GraphView Index::view() const {
     GraphView g;
     g.points = static_cast<const char*>(d_rows);
     g.row_type = row_type;
     g.nchunks = nchunks;
-    g.zero = d_zero;
-    g.upper = d_upper_ptrs;
-    g.n_upper = (uint32_t)d_upper.size();
+    g.zero = graph.zero;
+    g.upper = graph.upper_ptrs;
+    g.n_upper = (uint32_t)graph.upper.size();
     g.M = M;
     g.n = n;
     g.flags = opt_flags;
@@ -716,9 +687,6 @@ Index::~Index() {
     cudaFree(d_hdr);
     cudaFree(d_codes);
     cudaFree(d_cparams);
-    cudaFree(d_zero);
-    for (auto* p : d_upper) cudaFree(p);
-    cudaFree(d_upper_ptrs);
     cudaFree(d_id_map);
     for (auto& ln : lanes) ln.free_all();
     DeviceCtx::release(ctx);
@@ -750,69 +718,6 @@ idb_status Index::init_device(int dev) {
     if (const char* e = std::getenv("IDB_VIS_SLOTS")) vis_slots_override = next_pow2((uint64_t)std::max(64, std::atoi(e)));
     if (const char* e = std::getenv("IDB_SCREEN")) screen = std::atoi(e) != 0;
     if (const char* e = std::getenv("IDB_EXACT_SCRATCH_KEYS")) exact_scratch_keys = (uint64_t)std::max(1LL, std::atoll(e));
-    return IDB_OK;
-}
-
-idb_status Index::upload(uint64_t n_, uint32_t dim_, uint32_t M_, uint32_t ef, const uint32_t* zero, uint32_t n_upper,
-                         const uint32_t* const* upper, const uint64_t* upper_n_) {
-    // Layer l holds PointIds [0, n_l) (lib.rs:275-281): n >= n_1 >= n_2 >= ... >= 1.  The descent carries ids found on layer l
-    // into layer l-1 and seeds PointId 0 on the top layer, so anything else would read adjacency rows out of bounds.
-    for (uint32_t l = 0; l < n_upper; ++l) {
-        const uint64_t below = l == 0 ? n_ : upper_n_[l - 1];
-        if (upper_n_[l] == 0 || upper_n_[l] > below)
-            return fail(IDB_ERR_INVALID_ARG, "layer %u has %llu nodes but the layer below has %llu (need n >= n_1 >= ... >= 1)", l + 1,
-                        (unsigned long long)upper_n_[l], (unsigned long long)below);
-    }
-    n = n_;
-    cap = n_;
-    dim = dim_;
-    M = M_;
-    ef_search = ef;
-    nchunks = (dim + 3) / 4;
-    if (n == 0) return IDB_OK;
-    const size_t stride = (size_t)nchunks * 4;
-    if (n > SIZE_MAX / (stride * sizeof(float)) || n > SIZE_MAX / (2 * (size_t)M * 4)) return fail(IDB_ERR_INVALID_ARG, "n * dim overflows size_t");
-    CUDA_TRY(cudaMalloc(&d_zero, n * 2 * (size_t)M * 4));
-    if (zero) CUDA_TRY(cudaMemcpyAsync(d_zero, zero, n * 2 * (size_t)M * 4, cudaMemcpyHostToDevice, stream));
-    std::vector<const uint32_t*> ptrs;
-    for (uint32_t l = 0; l < n_upper; ++l) {
-        uint32_t* p = nullptr;
-        CUDA_TRY(cudaMalloc(&p, std::max<size_t>(4, upper_n_[l] * (size_t)M * 4)));
-        d_upper.push_back(p);
-        upper_n.push_back(upper_n_[l]);
-        if (upper && upper[l])
-            CUDA_TRY(cudaMemcpyAsync(p, upper[l], upper_n_[l] * (size_t)M * 4, cudaMemcpyHostToDevice, stream));
-        ptrs.push_back(p);
-    }
-    CUDA_TRY(cudaMalloc(&d_upper_ptrs, std::max<size_t>(1, n_upper) * sizeof(uint32_t*)));
-    if (n_upper)
-        CUDA_TRY(cudaMemcpyAsync(d_upper_ptrs, ptrs.data(), n_upper * sizeof(uint32_t*), cudaMemcpyHostToDevice, stream));
-    // reject graphs whose adjacency points outside the layer it belongs to
-    if (zero) {
-        uint32_t* d_bad = nullptr;
-        CUDA_TRY(cudaMalloc(&d_bad, 4));
-        CUDA_TRY(cudaMemsetAsync(d_bad, 0, 4, stream));
-        validate_rows_kernel<<<num_sms * 4, 256, 0, stream>>>(d_zero, n * 2 * (size_t)M, (uint32_t)n, d_bad);
-        for (uint32_t l = 0; l < n_upper; ++l)
-            if (upper && upper[l] && upper_n_[l])
-                validate_rows_kernel<<<num_sms * 4, 256, 0, stream>>>(d_upper[l], upper_n_[l] * (size_t)M, (uint32_t)upper_n_[l], d_bad);
-        uint32_t bad = 0;
-        cudaError_t e = cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-        if (e == cudaSuccess && bad == 0) {  // rows that list a PointId twice are legal input but rule out the b16 visited flavour
-            repeated_ids_kernel<<<num_sms * 8, 128, 0, stream>>>(d_zero, n, 2 * M, d_bad);
-            for (uint32_t l = 0; l < n_upper; ++l)
-                if (upper && upper[l] && upper_n_[l]) repeated_ids_kernel<<<num_sms * 8, 128, 0, stream>>>(d_upper[l], upper_n_[l], M, d_bad);
-            uint32_t rep = 0;
-            e = cudaMemcpyAsync(&rep, d_bad, 4, cudaMemcpyDeviceToHost, stream);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-            rows_distinct = rep == 0;
-        }
-        cudaFree(d_bad);
-        CUDA_TRY(e);
-        if (bad) return fail(IDB_ERR_INVALID_ARG, "%u adjacency entries refer to PointIds outside their layer", bad);
-    }
-    CUDA_TRY(cudaStreamSynchronize(stream));
     return IDB_OK;
 }
 
@@ -1022,9 +927,9 @@ idb_status idb_index_info(const idb_index* index, idb_info* out) {
     out->ef_search = ix->ef_search;
     out->device = ix->device;
     out->storage = ix->row_type;
-    out->n_layers = n == 0 ? 0 : (uint32_t)ix->d_upper.size() + 1;
+    out->n_layers = n == 0 ? 0 : (uint32_t)ix->graph.upper.size() + 1;
     if (n) out->layer_n[0] = n;
-    for (size_t l = 0; l < ix->upper_n.size() && l + 1 < 32; ++l) out->layer_n[l + 1] = ix->upper_n[l];
+    for (size_t l = 0; l < ix->graph.upper_n.size() && l + 1 < 32; ++l) out->layer_n[l + 1] = ix->graph.upper_n[l];
     return IDB_OK;
 }
 
@@ -1045,19 +950,17 @@ idb_status idb_index_export_zero(const idb_index* index, uint32_t* out) {
     if (ix->n == 0) return IDB_OK;
     std::lock_guard<std::mutex> lk(ix->mu);
     CUDA_TRY(cudaSetDevice(ix->device));
-    CUDA_TRY(cudaMemcpyAsync(out, ix->d_zero, ix->n * 2 * (size_t)ix->M * 4, cudaMemcpyDeviceToHost, ix->stream));
-    CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    CUDA_TRY(ix->graph.copy_out(0, 0, ix->n, ix->M, out, ix->stream));
     return IDB_OK;
 }
 
 idb_status idb_index_export_upper(const idb_index* index, uint32_t layer, uint32_t* out) {
     if (!index || !out) return fail(IDB_ERR_INVALID_ARG, "null argument");
     Index* ix = const_cast<Index*>(reinterpret_cast<const Index*>(index));
-    if (layer == 0 || layer > ix->d_upper.size()) return fail(IDB_ERR_INVALID_ARG, "layer %u out of range", layer);
-    std::lock_guard<std::mutex> lk(ix->mu);
+    std::lock_guard<std::mutex> lk(ix->mu);  // before the layer count: a removal can drop layers
+    if (layer == 0 || layer > ix->graph.upper.size()) return fail(IDB_ERR_INVALID_ARG, "layer %u out of range", layer);
     CUDA_TRY(cudaSetDevice(ix->device));
-    CUDA_TRY(cudaMemcpyAsync(out, ix->d_upper[layer - 1], ix->upper_n[layer - 1] * (size_t)ix->M * 4, cudaMemcpyDeviceToHost, ix->stream));
-    CUDA_TRY(cudaStreamSynchronize(ix->stream));
+    CUDA_TRY(ix->graph.copy_out(layer, 0, ix->graph.upper_n[layer - 1], ix->M, out, ix->stream));
     return IDB_OK;
 }
 

@@ -217,7 +217,7 @@ struct BatchRunner {
 
         std::memset(&a, 0, sizeof(a));
         a.g = ix->view();
-        a.zero = ix->d_zero;
+        a.zero = ix->graph.zero;
         a.efc = efc;
         a.cand_cap = cand_cap;
         a.keep_pruned = p.keep_pruned ? 1u : 0u;
@@ -361,19 +361,10 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
         return e;
     });
     if (s != IDB_OK) return s;
-    CUDA_TRY(cudaMalloc(&ix->d_zero, n * (size_t)cap * 4));
-    CUDA_TRY(fill_u32(ix->d_zero, n * (size_t)cap, kInvalid, st));
-    std::vector<const uint32_t*> ptrs;
-    for (uint32_t l = 1; l <= top; ++l) {
-        const uint64_t n_l = sizes[num_layers - 1 - l].second;
-        uint32_t* d = nullptr;
-        CUDA_TRY(cudaMalloc(&d, std::max<size_t>(4, n_l * (size_t)M * 4)));
-        ix->d_upper.push_back(d);
-        ix->upper_n.push_back(n_l);
-        ptrs.push_back(d);
-    }
-    CUDA_TRY(cudaMalloc(&ix->d_upper_ptrs, std::max<size_t>(1, top) * sizeof(uint32_t*)));
-    if (top) CUDA_TRY(cudaMemcpyAsync(ix->d_upper_ptrs, ptrs.data(), top * sizeof(uint32_t*), cudaMemcpyHostToDevice, st));
+    std::vector<uint64_t> upper_n;
+    for (uint32_t l = 1; l <= top; ++l) upper_n.push_back(sizes[num_layers - 1 - l].second);
+    CUDA_TRY(ix->graph.alloc(n, M, std::move(upper_n), st));
+    CUDA_TRY(fill_u32(ix->graph.zero, n * (size_t)cap, kInvalid, st));
 
     // ---- batch schedule + scratch -------------------------------------------------------------------------------
     uint32_t max_batch = 0, growth = 0;
@@ -397,7 +388,7 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
             if (p.progress) p.progress(g0, n, p.progress_user);  // set_position (core:519-525)
         }
         if (layer != 0) {  // lib.rs:323-328
-            snapshot_kernel<<<ix->num_sms * 4, 256, 0, st>>>(ix->d_zero, ix->d_upper[layer - 1], end, M);
+            snapshot_kernel<<<ix->num_sms * 4, 256, 0, st>>>(ix->graph.zero, ix->graph.upper[layer - 1], end, M);
             CUDA_TRY(cudaGetLastError());
         }
     }
@@ -457,6 +448,17 @@ idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_para
     return ix->build_codes();  // from all stored rows: the table's step, offsets and error bound follow the new rows
 }
 
+const char kNoExtendCandidates[] =
+    "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "
+    "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns";
+
+idb_status check_link_params(const idb_params* p) {
+    if (p->ef_construction == 0 || p->ef_construction > 1024)
+        return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", p->ef_construction);
+    if (p->heuristic && p->extend_candidates) return fail(IDB_ERR_UNSUPPORTED, "%s", kNoExtendCandidates);
+    return IDB_OK;
+}
+
 }  // namespace idb
 
 using namespace idb;
@@ -481,10 +483,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
     if (dim > 10240) return fail(IDB_ERR_UNSUPPORTED, "dim %u > 10240 is not supported (the owner row of a long-row traversal lives in shared memory)", dim);
     if (!(params->ml > 0.0f) || params->ml >= 1.0f) return fail(IDB_ERR_INVALID_ARG, "ml must be in (0, 1)");
     if (!storage_known(params->storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
-    if (params->heuristic && params->extend_candidates)
-        return fail(IDB_ERR_UNSUPPORTED,
-                    "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "
-                    "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns");
+    if (params->heuristic && params->extend_candidates) return fail(IDB_ERR_UNSUPPORTED, "%s", kNoExtendCandidates);
     auto* ix = new (std::nothrow) Index();
     if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");
     ix->metric = metric;
@@ -506,30 +505,18 @@ extern "C" idb_status idb_index_insert_f32(idb_index* index, const float* rows, 
     if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
     if (!params) return fail(IDB_ERR_INVALID_ARG, "params is null");
     if (m && !rows) return fail(IDB_ERR_INVALID_ARG, "rows is null");
-    if (params->ef_construction == 0 || params->ef_construction > 1024)
-        return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", params->ef_construction);
-    if (params->heuristic && params->extend_candidates)
-        return fail(IDB_ERR_UNSUPPORTED,
-                    "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "
-                    "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns");
-    idb_status st = require_device();
+    idb_status st = check_link_params(params);
+    if (st == IDB_OK) st = require_device();
     if (st != IDB_OK) return st;
     Index* ix = reinterpret_cast<Index*>(index);
-    // &mut self: no search, export or other insert runs while the index changes.  Every lane is taken (searches on other threads
-    // wait) and drained, so each search sees the index before or after this call.
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (auto& ln : ix->lanes) ln.mu.lock();
-    struct Unlock {
-        Index* ix;
-        ~Unlock() { for (auto& ln : ix->lanes) ln.mu.unlock(); }
-    } unlock{ix};
+    // &mut self: no search, export or other insert runs while the index changes, and each search sees it before or after this call
+    ExclusiveIndex ex(ix);
     if (dim != ix->dim) return fail(IDB_ERR_INVALID_ARG, "dim %u differs from the index's %u", dim, ix->dim);
     if (params->M != ix->M) return fail(IDB_ERR_INVALID_ARG, "M = %u differs from the index's %u", params->M, ix->M);
     if (m && ix->d_id_map && !global_ids) return fail(IDB_ERR_INVALID_ARG, "the index has an id map: global_ids is required");
     if (!ix->d_id_map && global_ids) return fail(IDB_ERR_INVALID_ARG, "global_ids given, but the index has no id map");
     if (ix->n + m >= 0xFFFFFFFFull)
         return fail(IDB_ERR_INVALID_ARG, "N = %llu + %llu >= u32::MAX (lib.rs:256)", (unsigned long long)ix->n, (unsigned long long)m);
-    CUDA_TRY(cudaSetDevice(ix->device));
-    for (auto& ln : ix->lanes) CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    CUDA_TRY(ex.drained);
     return insert_index(ix, rows, m, *params, global_ids, out_ids);
 }

@@ -7,6 +7,7 @@
 #include <functional>
 #include <mutex>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "../../include/instant_distance_b200.h"
@@ -224,6 +225,26 @@ __device__ __forceinline__ float stored_elem(const StoredRows& s, uint64_t r, ui
     return (h & 0x7fffu) > 0x7c00u ? __uint_as_float(((h & 0x8000u) << 16) | 0x7f800000u | ((h & 0x3ffu) << 13)) : widen_f16x2(h).x;
 }
 
+// An index's adjacency (DESIGN §2, graph.cu).  Move-only; frees what it holds.
+struct Graph {
+    uint32_t* zero = nullptr;                  // cap x 2M (rows past n: INVALID)
+    std::vector<uint32_t*> upper;              // [l-1] -> n_l x M
+    std::vector<uint64_t> upper_n;             // n >= n_1 >= ... >= 1
+    const uint32_t** upper_ptrs = nullptr;     // device copy of `upper` (GraphView::upper)
+    bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
+
+    Graph() = default;
+    Graph(Graph&& o) noexcept { *this = std::move(o); }
+    Graph& operator=(Graph&& o) noexcept;      // swaps: o frees what this held
+    ~Graph();
+    // On an empty Graph: zero of `cap` rows and one layer per entry of upper_n (contents unset), and the pointer table uploaded on st.
+    cudaError_t alloc(uint64_t cap, uint32_t M, std::vector<uint64_t> upper_n, cudaStream_t st);
+    // Rows [r0, r0 + m) of layer l (0 = zero) into host memory on st, then synchronises st.
+    cudaError_t copy_out(uint32_t l, uint64_t r0, uint64_t m, uint32_t M, uint32_t* host, cudaStream_t st) const;
+    // An adopted graph of n points: every entry INVALID or inside its layer (else IDB_ERR_INVALID_ARG), then rows_distinct.
+    idb_status check(uint64_t n, uint32_t M, int num_sms, cudaStream_t st);
+};
+
 struct Index {
     int device = 0;
     int num_sms = 132;
@@ -241,12 +262,8 @@ struct Index {
     float2* d_hdr = nullptr;                   // cap q8 row headers {o, s} (DESIGN §3c), else null
     uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as; set when the index is created
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
-    uint32_t* d_zero = nullptr;                // cap x 2M (rows past n: INVALID)
-    std::vector<uint32_t*> d_upper;            // [l-1] -> n_l x M
-    std::vector<uint64_t> upper_n;
-    const uint32_t** d_upper_ptrs = nullptr;   // device copy of the pointer table
+    Graph graph;
     uint32_t* d_id_map = nullptr;              // shard: PointId -> global row id (idb_index_set_id_map), cap entries
-    bool rows_distinct = true;                 // no adjacency row lists a PointId twice (checked for adopted graphs)
     // Screening table of the stored rows (DESIGN §2, §4): n x code_words(nchunks) u32 of 8-bit codes (zero padded to a multiple of
     // 16 bytes) + 3 x nchunks float4 (scale, offset, E),
     // one code step for every element and the bound on every row's coding error (GraphView::cstep / cerr).
@@ -277,8 +294,8 @@ struct Index {
 
     ~Index();
     idb_status init_device(int dev);
-    // The graph of an index of n rows (cap = n): layer sizes checked, zero and upper allocated (and copied when given), adjacency
-    // entries checked.  The rows are put in by the caller (put_rows).
+    // The graph of an index of n rows (cap = n, graph.cu): layer sizes checked, zero and upper allocated and copied (each upper layer
+    // when given), adjacency entries checked.  The rows are put in by the caller (put_rows).
     idb_status upload(uint64_t n, uint32_t dim, uint32_t M, uint32_t ef, const uint32_t* zero, uint32_t n_upper,
                       const uint32_t* const* upper, const uint64_t* upper_n);
     GraphView view() const;
@@ -299,7 +316,8 @@ struct Index {
     cudaError_t alloc_rows(uint64_t rows, void** pts, float2** hdr) const;  // a store of `rows` rows (and q8 headers); frees nothing
     idb_status copy_points_f32(float* host_out, uint64_t r0, uint64_t m);  // rows [r0, r0+m) widened to m x dim f32 on the host
     // ----
-    // The zero rows of rows [r0, r0 + m) INVALID, and global_ids (m entries) into the id map when it exists (the insert, after put_rows).
+    // The zero rows of rows [r0, r0 + m) INVALID, and global_ids (m entries) into the id map when it exists (the insert, after
+    // put_rows; graph.cu).
     idb_status stage_rows(uint64_t r0, uint64_t m, const uint32_t* global_ids);
     idb_status build_codes();                                            // (re)builds d_codes / d_cparams from the stored rows
     int search_grid() const;
@@ -324,6 +342,23 @@ struct Index {
     // run none.  `latest`: lane 0xFFFFFFFF names the lane of the last call issued on this index.
     idb_status last_search(uint32_t lane, bool latest, SearchCtrl* ctrl, uint32_t* kernel);
 };
+
+// The index held exclusively (&mut self) by a call that changes it (insert, remove, set_id_map): its mutex, then every lane's, in
+// that order, so searches on other threads wait; then the index's device is set and every lane's stream drained, so what they
+// enqueued before (and reads on the device) has run.  `drained` is that step's result, for the caller to report.
+struct ExclusiveIndex {
+    Index* ix;
+    cudaError_t drained;
+    explicit ExclusiveIndex(Index* index);
+    ~ExclusiveIndex();
+    ExclusiveIndex(const ExclusiveIndex&) = delete;
+    ExclusiveIndex& operator=(const ExclusiveIndex&) = delete;
+};
+
+// The linking parameters of an insert or a removal: ef_construction in 1..1024, and no extend_candidates with the heuristic
+// (IDB_ERR_UNSUPPORTED).  kNoExtendCandidates is the refusal's message, which the build shares.
+extern const char kNoExtendCandidates[];
+idb_status check_link_params(const idb_params* p);
 
 constexpr uint32_t kExactMaxK = 1024;  // the exact search's largest k
 

@@ -51,16 +51,16 @@ idb_status idb_index_save(const idb_index* index, const char* path) {
     std::vector<uint32_t> rows((size_t)chunk * 2 * ix->M);
     for (uint64_t r0 = 0; ok && r0 < n; r0 += chunk) {
         const uint64_t m = std::min(chunk, n - r0);
-        CUDA_TRY(cudaMemcpy(rows.data(), ix->d_zero + r0 * 2 * ix->M, m * 2 * ix->M * 4, cudaMemcpyDeviceToHost));
+        CUDA_TRY(ix->graph.copy_out(0, r0, m, ix->M, rows.data(), ix->stream));
         ok = put(out.f, rows.data(), m * 2 * ix->M * 4);
     }
     // layers: Vec<Vec<UpperNode>>, layers[0] = layer 1
-    ok = ok && put_u64(out.f, ix->d_upper.size());
-    for (size_t l = 0; ok && l < ix->d_upper.size(); ++l) {
-        const uint64_t nl = ix->upper_n[l];
+    ok = ok && put_u64(out.f, ix->graph.upper.size());
+    for (uint32_t l = 1; ok && l <= ix->graph.upper.size(); ++l) {
+        const uint64_t nl = ix->graph.upper_n[l - 1];
         ok = put_u64(out.f, nl);
         std::vector<uint32_t> u((size_t)nl * ix->M);
-        if (nl) CUDA_TRY(cudaMemcpy(u.data(), ix->d_upper[l], nl * ix->M * 4, cudaMemcpyDeviceToHost));
+        CUDA_TRY(ix->graph.copy_out(l, 0, nl, ix->M, u.data(), ix->stream));
         ok = ok && put(out.f, u.data(), u.size() * 4);
     }
     if (!ok) return fail(IDB_ERR_IO, "short write to %s", path);

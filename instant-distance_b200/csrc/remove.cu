@@ -248,7 +248,8 @@ __global__ void relabel_rows_kernel(const uint32_t* new_ids, uint64_t n_rows, ui
     }
 }
 
-// Every device buffer of one removal, allocated before anything is written; what is not handed to the index is freed.
+// The device buffers of one removal other than its compacted graph (a Graph of its own), allocated before anything is written; what
+// is not handed to the index is freed.
 struct RemoveBuffers {
     uint32_t* removed = nullptr;
     uint32_t* keep = nullptr;
@@ -257,15 +258,10 @@ struct RemoveBuffers {
     void* cub_tmp = nullptr;
     void* rows = nullptr;
     float2* hdr = nullptr;
-    uint32_t* zero = nullptr;
     uint32_t* id_map = nullptr;
-    std::vector<uint32_t*> upper;
-    const uint32_t** upper_ptrs = nullptr;
     ~RemoveBuffers() {
         cudaFree(removed); cudaFree(keep); cudaFree(new_ids); cudaFree(work); cudaFree(cub_tmp);
-        cudaFree(rows); cudaFree(hdr); cudaFree(zero); cudaFree(id_map);
-        for (auto* u : upper) cudaFree(u);
-        cudaFree(upper_ptrs);
+        cudaFree(rows); cudaFree(hdr); cudaFree(id_map);
     }
 };
 
@@ -278,7 +274,7 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
         return IDB_OK;
     }
     cudaStream_t st = ix->stream;
-    const uint32_t M = ix->M, n_layers = (uint32_t)ix->d_upper.size() + 1;
+    const uint32_t M = ix->M, n_layers = (uint32_t)ix->graph.upper.size() + 1;
     const uint64_t n1 = n - m, cap1 = std::max<uint64_t>(n1, 1);
     // ---- host: the bitmap of R and the surviving layer sizes (per removed id, never per row) ---------------------------------------
     const uint64_t words = (n + 31) / 32;
@@ -287,11 +283,12 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
     std::vector<uint64_t> upper_n1(n_layers - 1);
     for (uint32_t l = 1; l < n_layers; ++l) {
         uint64_t below = 0;
-        for (uint64_t i = 0; i < m; ++i) below += pids[i] < ix->upper_n[l - 1] ? 1u : 0u;
-        upper_n1[l - 1] = ix->upper_n[l - 1] - below;
+        for (uint64_t i = 0; i < m; ++i) below += pids[i] < ix->graph.upper_n[l - 1] ? 1u : 0u;
+        upper_n1[l - 1] = ix->graph.upper_n[l - 1] - below;
     }
     uint32_t layers1 = 1;  // layers left: the upper layers that keep a point
     while (layers1 < n_layers && upper_n1[layers1 - 1] > 0) ++layers1;
+    upper_n1.resize(layers1 - 1);
 
     // ---- every buffer first: a failed allocation leaves the index as it was ----------------------------------------------------------
     RemoveBuffers b;
@@ -304,14 +301,10 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
     CUDA_TRY(cudaMalloc(&b.new_ids, n * 4));
     CUDA_TRY(cudaMalloc(&b.work, n_layers * sizeof(unsigned long long)));
     CUDA_TRY(ix->alloc_rows(cap1, &b.rows, &b.hdr));
-    CUDA_TRY(cudaMalloc(&b.zero, cap1 * 2 * (size_t)M * 4));
+    Graph next;  // the compacted graph; once swapped in, it frees the old layers, the dropped ones included
+    CUDA_TRY(next.alloc(cap1, M, std::move(upper_n1), st));
+    next.rows_distinct = ix->graph.rows_distinct;  // repaired rows come from distinct keys, and the relabelling is injective
     if (ix->d_id_map) CUDA_TRY(cudaMalloc(&b.id_map, cap1 * 4));
-    for (uint32_t l = 1; l < layers1; ++l) {
-        uint32_t* u = nullptr;
-        CUDA_TRY(cudaMalloc(&u, upper_n1[l - 1] * (size_t)M * 4));
-        b.upper.push_back(u);
-    }
-    CUDA_TRY(cudaMalloc(&b.upper_ptrs, std::max<size_t>(1, layers1 - 1) * sizeof(uint32_t*)));
 
     // ---- repair every layer in place ------------------------------------------------------------------------------------------------
     CUDA_TRY(cudaMemcpyAsync(b.removed, bits.data(), words * 4, cudaMemcpyHostToDevice, st));
@@ -329,8 +322,8 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
     a.heuristic = p.heuristic ? 1u : 0u;
     a.keep_pruned = p.keep_pruned ? 1u : 0u;
     for (uint32_t l = 0; l < n_layers; ++l) {
-        a.rows = l == 0 ? ix->d_zero : ix->d_upper[l - 1];
-        a.n_rows = l == 0 ? n : ix->upper_n[l - 1];
+        a.rows = l == 0 ? ix->graph.zero : ix->graph.upper[l - 1];
+        a.n_rows = l == 0 ? n : ix->graph.upper_n[l - 1];
         a.width = l == 0 ? 2 * M : M;
         a.work = b.work + l;
         const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((a.n_rows + kBuildWarps - 1) / kBuildWarps, (uint64_t)ix->num_sms * ctas_per_sm));
@@ -344,30 +337,24 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(b.cub_tmp, cub_bytes, b.keep, b.new_ids, (int64_t)n, st));
     drop_removed_kernel<<<blocks, 256, 0, st>>>(b.removed, n, b.new_ids);
     CUDA_TRY(cudaGetLastError());
-    if (n1 == 0) CUDA_TRY(fill_u32(b.zero, 2 * (size_t)M, kInvalid, st));  // the one row of an empty store
+    if (n1 == 0) CUDA_TRY(fill_u32(next.zero, 2 * (size_t)M, kInvalid, st));  // the one row of an empty store
     compact_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, (uint32_t)(ix->row_bytes() / 4), static_cast<const uint32_t*>(ix->d_rows),
                                                 static_cast<uint32_t*>(b.rows), ix->d_hdr, b.hdr, ix->d_id_map, b.id_map);
     CUDA_TRY(cudaGetLastError());
-    relabel_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, 2 * M, ix->d_zero, b.zero);
+    relabel_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, 2 * M, ix->graph.zero, next.zero);
     CUDA_TRY(cudaGetLastError());
     for (uint32_t l = 1; l < layers1; ++l) {
-        relabel_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, ix->upper_n[l - 1], M, ix->d_upper[l - 1], b.upper[l - 1]);
+        relabel_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, ix->graph.upper_n[l - 1], M, ix->graph.upper[l - 1], next.upper[l - 1]);
         CUDA_TRY(cudaGetLastError());
     }
-    if (layers1 > 1)
-        CUDA_TRY(cudaMemcpyAsync(b.upper_ptrs, b.upper.data(), (layers1 - 1) * sizeof(uint32_t*), cudaMemcpyHostToDevice, st));
     if (out_new_ids) CUDA_TRY(cudaMemcpyAsync(out_new_ids, b.new_ids, n * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
 
     // ---- swap in ------------------------------------------------------------------------------------------------------------------------
     std::swap(ix->d_rows, b.rows);
     std::swap(ix->d_hdr, b.hdr);
-    std::swap(ix->d_zero, b.zero);
     std::swap(ix->d_id_map, b.id_map);
-    std::swap(ix->d_upper, b.upper);  // the old layers are freed with b, the dropped ones included
-    std::swap(ix->d_upper_ptrs, b.upper_ptrs);
-    upper_n1.resize(layers1 - 1);
-    ix->upper_n = upper_n1;
+    std::swap(ix->graph, next);
     ix->cap = cap1;
     ix->n = n1;
     return ix->build_codes();  // from the stored rows that remain
@@ -385,22 +372,11 @@ extern "C" idb_status idb_index_remove(idb_index* index, const uint32_t* pids, u
     if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
     if (!params) return fail(IDB_ERR_INVALID_ARG, "params is null");
     if (m && !pids) return fail(IDB_ERR_INVALID_ARG, "pids is null");
-    if (params->ef_construction == 0 || params->ef_construction > 1024)
-        return fail(IDB_ERR_UNSUPPORTED, "ef_construction = %u unsupported (1..1024)", params->ef_construction);
-    if (params->heuristic && params->extend_candidates)
-        return fail(IDB_ERR_UNSUPPORTED,
-                    "Heuristic::extend_candidates = true is not supported: in the reference it re-locks the row being inserted "
-                    "(lib.rs:438 write lock vs lib.rs:649 read lock through types.rs:146) and never returns");
-    idb_status st = require_device();
+    idb_status st = check_link_params(params);
+    if (st == IDB_OK) st = require_device();
     if (st != IDB_OK) return st;
     Index* ix = reinterpret_cast<Index*>(index);
-    // &mut self, as the insert: every lane is taken and drained, so each search on another thread sees the index before or after
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (auto& ln : ix->lanes) ln.mu.lock();
-    struct Unlock {
-        Index* ix;
-        ~Unlock() { for (auto& ln : ix->lanes) ln.mu.unlock(); }
-    } unlock{ix};
+    ExclusiveIndex ex(ix);  // &mut self, as the insert: each search on another thread sees the index before or after
     if (params->M != ix->M) return fail(IDB_ERR_INVALID_ARG, "M = %u differs from the index's %u", params->M, ix->M);
     const uint64_t n = ix->n;
     std::vector<uint32_t> seen((n + 31) / 32, 0u);
@@ -416,7 +392,6 @@ extern "C" idb_status idb_index_remove(idb_index* index, const uint32_t* pids, u
         }
         seen[x >> 5] |= 1u << (x & 31);
     }
-    CUDA_TRY(cudaSetDevice(ix->device));
-    for (auto& ln : ix->lanes) CUDA_TRY(cudaStreamSynchronize(ln.stream));
+    CUDA_TRY(ex.drained);
     return remove_index(ix, pids, m, *params, out_new_ids);
 }

@@ -222,7 +222,7 @@ idb_status Index::reserve_rows(uint64_t rows) {
     const size_t row_bytes = (size_t)nchunks * 4 * elem_bytes(row_type), width = 2 * (size_t)M;
     void* pts = nullptr;
     float2* hdr = nullptr;
-    uint32_t* zero = nullptr;
+    uint32_t* zero = nullptr;  // the one adjacency layer allocated outside graph.cu: it grows with the rows, all or nothing
     uint32_t* id_map = nullptr;
     cudaError_t e = alloc_store(*this, want, &pts, &hdr);
     if (e == cudaSuccess) e = cudaMalloc(&zero, want * width * 4);
@@ -230,7 +230,7 @@ idb_status Index::reserve_rows(uint64_t rows) {
     if (e == cudaSuccess && n) {
         e = cudaMemcpyAsync(pts, d_rows, n * row_bytes, cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess && hdr) e = cudaMemcpyAsync(hdr, d_hdr, n * sizeof(float2), cudaMemcpyDeviceToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(zero, d_zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(zero, graph.zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(id_map, d_id_map, n * 4, cudaMemcpyDeviceToDevice, stream);
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
@@ -243,11 +243,11 @@ idb_status Index::reserve_rows(uint64_t rows) {
     }
     cudaFree(d_rows);
     cudaFree(d_hdr);
-    cudaFree(d_zero);
+    cudaFree(graph.zero);
     cudaFree(d_id_map);
     d_rows = pts;
     d_hdr = hdr;
-    d_zero = zero;
+    graph.zero = zero;
     d_id_map = id_map;
     cap = want;
     return IDB_OK;

@@ -109,8 +109,8 @@ void idb_comm_free(idb_comm* comm) {
 idb_status idb_index_set_id_map(idb_index* index, const uint32_t* global_ids) {
     if (!index) return fail(IDB_ERR_INVALID_ARG, "index is null");
     Index* ix = reinterpret_cast<Index*>(index);
-    std::lock_guard<std::mutex> lk(ix->mu);
-    CUDA_TRY(cudaSetDevice(ix->device));
+    ExclusiveIndex ex(ix);  // searches read the map on the device: none may run on any lane while it changes
+    CUDA_TRY(ex.drained);
     if (!global_ids) {
         cudaFree(ix->d_id_map);
         ix->d_id_map = nullptr;
