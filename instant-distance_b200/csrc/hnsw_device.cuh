@@ -264,21 +264,38 @@ template <bool kDown>
 __device__ __forceinline__ float fadd_dir(float a, float b) { return kDown ? __fadd_rd(a, b) : __fadd_rn(a, b); }
 template <bool kDown>
 __device__ __forceinline__ uint32_t fadd_dir(uint32_t a, uint32_t b) { return a + b; }
+// c ? a : b as one SELP on the two values: a C++ `up ? p[2i] : p[2i+1]` may be folded into one load from a selected address, which
+// indexes p at run time and puts it on the stack.
+__device__ __forceinline__ float sel(bool c, float a, float b) {
+    float r;
+    asm("{ .reg .pred p; setp.ne.u32 p, %3, 0; selp.f32 %0, %1, %2, p; }" : "=f"(r) : "f"(a), "f"(b), "r"((uint32_t)c));
+    return r;
+}
+__device__ __forceinline__ uint32_t sel(bool c, uint32_t a, uint32_t b) {
+    uint32_t r;
+    asm("{ .reg .pred p; setp.ne.u32 p, %3, 0; selp.b32 %0, %1, %2, p; }" : "=r"(r) : "r"(a), "r"(b), "r"((uint32_t)c));
+    return r;
+}
+// The transposing stage at offset OFF, M vectors left, and the stages after it.  One template per stage, so that every loop below
+// has a constant trip count: as one loop nest over m, the inner loop (trip count m / 2) was unrolled by four before m was known,
+// which indexed p at run time and put it on the stack (64 bytes at NB = 16).
+template <int M, int OFF, bool kDown, class T, int NB>
+__device__ __forceinline__ void butterfly_stages(T (&p)[NB], int lane) {
+    if constexpr (M > 1) {
+        const bool up = (lane & OFF) != 0;
+#pragma unroll
+        for (int i = 0; i < M / 2; ++i) {
+            const T send = sel(up, p[2 * i], p[2 * i + 1]);
+            const T keep = sel(up, p[2 * i + 1], p[2 * i]);
+            p[i] = fadd_dir<kDown>(keep, __shfl_xor_sync(kFullMask, send, OFF));
+        }
+        butterfly_stages<M / 2, 2 * OFF, kDown>(p, lane);
+    }
+}
 template <int NB, bool kDown = false, class T = float, int W = 32>
 __device__ __forceinline__ T batch_butterfly(T (&p)[NB], int lane) {
     static_assert(NB <= W, "one vector per lane of a group at most");
-    int off = 1;
-#pragma unroll
-    for (int m = NB; m > 1; m >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < m / 2; ++i) {
-            T send = up ? p[2 * i] : p[2 * i + 1];
-            T keep = up ? p[2 * i + 1] : p[2 * i];
-            p[i] = fadd_dir<kDown>(keep, __shfl_xor_sync(kFullMask, send, off));
-        }
-        off <<= 1;
-    }
+    butterfly_stages<NB, 1, kDown>(p, lane);
 #pragma unroll
     for (int o = NB; o < W; o <<= 1) p[0] = fadd_dir<kDown>(p[0], __shfl_xor_sync(kFullMask, p[0], o));
     return p[0];
@@ -667,8 +684,8 @@ __device__ __forceinline__ bool vis_reserve(VisitedSet& v, uint32_t incoming, in
 #ifdef IDB_K1_PHASES
 enum K1Phase : int {
     kPhPop, kPhAdj, kPhVisit, kPhScreenLoad, kPhScreenMath, kPhGather, kPhMerge, kPhTies, kPhCount,
-    // event counts behind the cycle tallies
-    kPhExpansions = kPhCount, kPhScreenBatches, kPhSlots
+    // event counts behind the cycle tallies; dist_*: batch_distances_impl's batches, the row slots they load, the rows they hold
+    kPhExpansions = kPhCount, kPhScreenBatches, kPhDistBatches, kPhDistSlots, kPhDistRows, kPhSlots
 };
 static __device__ unsigned long long g_k1_phases[kPhSlots];
 #define IDB_PHASE(s, k) k1_phase_mark(s, k)
@@ -738,7 +755,69 @@ __device__ __forceinline__ uint32_t lower_bound_keys(const uint64_t* a, uint32_t
     return lo;
 }
 
-// Distances from q to the n_new points listed in cpid (shared, 16-byte aligned), NB rows in flight per lane; writes the
+// The width ladder of batch_distances_impl.  Since the screen, an expansion fetches a handful of rows (DESIGN §5), so most batches
+// are the last, part-filled one; a batch costs instructions for every slot, used or not.  So a batch is NB rows wide while NB rows
+// are left, and the last one takes the narrowest of NB, NB/2, ..., FLOOR that holds every row left.  FLOOR (batch_floor) is the
+// narrowest batch that still keeps four chunk loads and two rows in flight per lane.  A row's sum does not depend on the width
+// (batch_butterfly), so neither does any key.
+template <int CH>
+__host__ __device__ constexpr int batch_floor() { return (4 + CH - 1) / CH > 2 ? (4 + CH - 1) / CH : 2; }
+// The width of the next batch when rest >= 1 rows are left.
+template <int NB, int FLOOR>
+__host__ __device__ constexpr int batch_width(uint32_t rest) {
+    int w = NB;
+    while (w > FLOOR && rest <= (uint32_t)(w / 2)) w /= 2;
+    return w;
+}
+
+// One batch of batch_distances_impl: rows b0 .. b0 + min(nb, NB) - 1 of cpid, NB rows in flight per lane.
+template <int CH, int NB, bool kFull, class RT>
+__device__ __forceinline__ void distance_batch(const GraphView& g, const float4 (&q)[CH], const uint32_t* cpid, uint64_t* ckey,
+                                               uint32_t b0, uint32_t nb, const char* lane_base, uint32_t row_bytes,
+                                               const bool (&cok)[CH], int lane) {
+    typename RT::Raw v[NB][CH];
+    typename RT::Hdr h[NB];
+    if (kFull && nb >= (uint32_t)NB) {  // uniform; plain loads, no predicates, no zero fill
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
+            h[i] = RT::hdr(g, cpid[b0 + i]);
+#pragma unroll
+            for (int j = 0; j < CH; ++j) v[i][j] = RT::ld_raw(row + j * 32 * RT::kChunkBytes);
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            // branch-free on purpose: `if (i < nb) {load; use}` makes ptxas emit two branches per row
+            const bool ok = (uint32_t)i < nb;
+            const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
+            h[i] = ok ? RT::hdr(g, cpid[b0 + i]) : typename RT::Hdr();
+#pragma unroll
+            for (int j = 0; j < CH; ++j)
+                v[i][j] = (ok && cok[j]) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
+        }
+    }
+    float p[NB];
+#pragma unroll
+    for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(g, q, v[i], h[i], lane);
+    const float total = batch_butterfly<NB>(p, lane);
+    if ((uint32_t)lane < nb && lane < NB) ckey[b0 + lane] = mk_key(total, cpid[b0 + lane]);
+}
+// distance_batch at width w, one of NB, NB/2, ..., FLOOR (warp-uniform).
+template <int CH, int NB, int FLOOR, bool kFull, class RT>
+__device__ __forceinline__ void distance_batch_at(int w, const GraphView& g, const float4 (&q)[CH], const uint32_t* cpid,
+                                                  uint64_t* ckey, uint32_t b0, uint32_t nb, const char* lane_base, uint32_t row_bytes,
+                                                  const bool (&cok)[CH], int lane) {
+    if constexpr (NB > FLOOR) {
+        if (w < NB) {
+            distance_batch_at<CH, NB / 2, FLOOR, kFull, RT>(w, g, q, cpid, ckey, b0, nb, lane_base, row_bytes, cok, lane);
+            return;
+        }
+    }
+    distance_batch<CH, NB, kFull, RT>(g, q, cpid, ckey, b0, nb, lane_base, row_bytes, cok, lane);
+}
+
+// Distances from q to the n_new points listed in cpid (shared, 16-byte aligned), up to NB rows in flight per lane; writes the
 // keys (canonical distance bits << 32 | pid) to ckey.  The only place in the traversal that touches point rows.
 // kFull: every lane owns a real chunk in every one of its CH slots (dim is a multiple of 128) -> no chunk predicates.
 template <int CH, int NB, bool kFull, class RT>
@@ -758,36 +837,11 @@ __device__ __forceinline__ void batch_distances_impl(const GraphView& g, const f
     bool cok[CH];
 #pragma unroll
     for (int j = 0; j < CH; ++j) cok[j] = kFull || (uint32_t)(lane + 32 * j) < g.nchunks;
+    constexpr int FLOOR = batch_floor<CH>();
 #pragma unroll 1
-    for (uint32_t b0 = 0; b0 < n_new; b0 += NB) {
-        const uint32_t nb = n_new - b0;  // rows in this batch (uniform); entries i >= nb are predicated off
-        typename RT::Raw v[NB][CH];
-        typename RT::Hdr h[NB];
-        if (kFull && nb >= (uint32_t)NB) {  // uniform; two of the ~three trips per expansion: plain loads, no predicates, no zero fill
-#pragma unroll
-            for (int i = 0; i < NB; ++i) {
-                const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
-                h[i] = RT::hdr(g, cpid[b0 + i]);
-#pragma unroll
-                for (int j = 0; j < CH; ++j) v[i][j] = RT::ld_raw(row + j * 32 * RT::kChunkBytes);
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < NB; ++i) {
-                // branch-free on purpose: `if (i < nb) {load; use}` makes ptxas emit two branches per row
-                const bool ok = (uint32_t)i < nb;
-                const char* row = lane_base + (size_t)cpid[b0 + i] * row_bytes;  // shared-memory broadcast of the id
-                h[i] = ok ? RT::hdr(g, cpid[b0 + i]) : typename RT::Hdr();
-#pragma unroll
-                for (int j = 0; j < CH; ++j)
-                    v[i][j] = (ok && cok[j]) ? RT::ld_raw(row + j * 32 * RT::kChunkBytes) : RT::zero();
-            }
-        }
-        float p[NB];
-#pragma unroll
-        for (int i = 0; i < NB; ++i) p[i] = lane_partial_raw<CH, RT>(g, q, v[i], h[i], lane);
-        const float total = batch_butterfly<NB>(p, lane);
-        if ((uint32_t)lane < nb && lane < NB) ckey[b0 + lane] = mk_key(total, cpid[b0 + lane]);
+    for (uint32_t b0 = 0, w; b0 < n_new; b0 += w) {
+        w = (uint32_t)batch_width<NB, FLOOR>(n_new - b0);  // uniform; rows i >= n_new - b0 of the batch are predicated off
+        distance_batch_at<CH, NB, FLOOR, kFull, RT>((int)w, g, q, cpid, ckey, b0, n_new - b0, lane_base, row_bytes, cok, lane);
     }
     __syncwarp();
 }
@@ -1257,6 +1311,16 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
         // ---- distances (lib.rs:709-710) --------------------------------------------------------------------
         if constexpr (TMA) batch_distances_tma<CH, B>(g, q.r, s.cpid, s.ckey, n_new, lane, s);
         else batch_distances<CH, B, RT, FULL>(g, q, s.cpid, s.ckey, n_new, lane);
+#ifdef IDB_K1_PHASES
+        if constexpr (CH > 0 && !TMA) {
+            for (uint32_t b0 = 0, w; b0 < n_new; b0 += w) {
+                w = (uint32_t)batch_width<B, batch_floor<CH>()>(n_new - b0);
+                IDB_PHASE_COUNT(s, kPhDistBatches, 1u);
+                IDB_PHASE_COUNT(s, kPhDistSlots, w);
+            }
+            IDB_PHASE_COUNT(s, kPhDistRows, n_new);
+        }
+#endif
         uint64_t keyg[ROW_T];
 #pragma unroll
         for (int gi = 0; gi < ROW_T; ++gi) {

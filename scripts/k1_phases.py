@@ -23,7 +23,7 @@ CSRC = os.path.join(ROOT, "instant-distance_b200", "csrc")
 HEADLINE = "_ZN3idb13search_kernelILi1ELi2ELi4ELi16ELi4ENS_6RowF32ELb1ELb0EEEvNS_10SearchArgsE"
 # order of K1Phase in hnsw_device.cuh
 PHASES = ["pop", "adjacency_load", "visited_probe_commit", "screen_loads", "screen_math", "gather_and_distances", "admission_merge", "ties"]
-EVENTS = ["expansions", "screen_batches"]
+EVENTS = ["expansions", "screen_batches", "distance_batches", "distance_row_slots", "distance_rows"]
 
 
 def sass_counts(lib):
@@ -118,6 +118,11 @@ def main():
         "phase_share": {k: x / max(1, total) for k, x in cyc.items()},
         "phase_cycles_per_expansion": {k: x / max(1, ev["expansions"]) for k, x in cyc.items()},
         "screen_batches_per_expansion": ev["screen_batches"] / max(1, ev["expansions"]),
+        # batch_distances_impl: batches, row slots loaded and rows used (the slots past the rows are predicated off)
+        "distance_batches_per_expansion": ev["distance_batches"] / max(1, ev["expansions"]),
+        "distance_rows_per_expansion": ev["distance_rows"] / max(1, ev["expansions"]),
+        "distance_row_slots_per_expansion": ev["distance_row_slots"] / max(1, ev["expansions"]),
+        "distance_rows_per_slot": ev["distance_rows"] / max(1, ev["distance_row_slots"]),
     }), flush=True)
 
 
