@@ -41,6 +41,14 @@ extern "C" {
  * is refused with IDB_ERR_INVALID_ARG, naming its row and element, before the index changes.  A q8 index has no screening table.
  * (The value 3 is not a storage.) */
 #define IDB_STORAGE_Q8 4u
+/* Binary rows (DESIGN.md §3d): every element is 0 or 1, kept as one bit in one byte per 4 elements (element 4c + k is bit k of byte c,
+ * the high nibble zero), a sixteenth of the f32 bytes.  A row element must be +0.0, -0.0 (stored as 0) or 1.0; any other value (0.5, 2,
+ * -1, NaN, +-inf, a subnormal) is refused with IDB_ERR_INVALID_ARG, naming its row and element, before the index changes.  Metric
+ * IDB_METRIC_L2SQ only (IDB_METRIC_COSINE with bin: IDB_ERR_UNSUPPORTED, normalised rows are not 0/1).  Queries are any f32 rows and
+ * the reported distance is the canonical squared L2 to the 0/1 row; for a 0/1 query every partial sum is a small integer, so it is
+ * exactly the Hamming distance.  Packed codes (8 elements per byte, most significant bit first) become queries and rows with
+ * np.unpackbits(codes, axis=1).astype(np.float32).  A bin index has no screening table.  (The values 5 to 7 are not storages.) */
+#define IDB_STORAGE_BIN 8u
 /* Metrics (DESIGN.md §3a).  IDB_METRIC_COSINE: every row and every query is normalised in the canonical order (x / sqrt(sum x^2),
  * correctly rounded; a row whose sum of squares overflows becomes zeros and NaN), the traversal runs the canonical squared L2 on
  * the normalised rows, and the reported distance is half of it: 1 - cos(x, y) (0 .. 2).  An all-zero row stays zero, so it is at
@@ -87,8 +95,9 @@ typedef struct idb_params {
     int32_t  device;            /* CUDA device ordinal */
     uint32_t storage;           /* IDB_STORAGE_F32 (default), IDB_STORAGE_BF16 or IDB_STORAGE_F16: rows rounded to bf16 / fp16 (RNE)
                                    and kept in HBM at half the bytes; IDB_STORAGE_Q8: rows quantised to a per-row 8-bit grid, a
-                                   quarter of the bytes plus 8 bytes per row.  Distances still accumulate in fp32 in the same
-                                   canonical order.  An index with no rows records it for the rows a later insert adds. */
+                                   quarter of the bytes plus 8 bytes per row; IDB_STORAGE_BIN: 0/1 rows at one byte per four
+                                   elements.  Distances still accumulate in fp32 in the same canonical order.  An index with no
+                                   rows records it for the rows a later insert adds. */
     /* Builder::progress(ProgressBar) (core:70-75; feature `indicatif`): called on the building thread with the number of
      * points whose insertion has been enqueued so far (set_position, core:519-525) and the total (set_length, core:216-222);
      * the last call has done == total (finish, core:331-334).  NULL = no reporting. */
@@ -178,7 +187,8 @@ IDB_API idb_status idb_index_from_graph_bf16(const float* points, uint64_t n, ui
                                      const uint64_t* upper_n, int32_t device, idb_index** out_index);
 
 /* Both of the above and the metric: storage = IDB_STORAGE_* (IDB_STORAGE_F16: the rows rounded to fp16, IDB_STORAGE_Q8: the rows
- * quantised; results equal the reference algorithm run on the rounded or dequantised points), metric = IDB_METRIC_*.  With IDB_METRIC_COSINE the points are taken as given
+ * quantised, IDB_STORAGE_BIN: 0/1 rows, refused with IDB_METRIC_COSINE as IDB_ERR_UNSUPPORTED; results equal the reference
+ * algorithm run on the rounded or dequantised points), metric = IDB_METRIC_*.  With IDB_METRIC_COSINE the points are taken as given
  * (normalising is not idempotent bit for bit, so an adopted graph keeps the exact rows it was built on): every row must be all zeros
  * or have |sum x^2 - 1| <= 1e-2 (which lets bf16- and fp16-rounded and q8-quantised unit rows through), else IDB_ERR_INVALID_ARG.
  * idb_normalize_f32 gives the canonical normalisation. */
@@ -274,7 +284,7 @@ IDB_API idb_status idb_last_search_retried(idb_index* index, uint32_t lane, uint
 IDB_API idb_status idb_last_search_full_fetches(idb_index* index, uint32_t lane, uint64_t* out_rows);
 /* Diagnostics: which instantiation of the search kernel the last call on `lane` launched (its main pass; the retry pass uses the same
  * one).  out (8 u32) = {CH (float4 chunks per lane of a row, 0 = the long-row kernel), ROW_T, EF_T, B (rows in flight per lane), the
- * row type (IDB_STORAGE_*: 0 f32, 1 bf16, 2 fp16, 4 q8), 1 if FULL (no chunk predicates), 1 if TMA, the IDB_VARIANT case taken (0 = the
+ * row type (IDB_STORAGE_*: 0 f32, 1 bf16, 2 fp16, 4 q8, 8 bin), 1 if FULL (no chunk predicates), 1 if TMA, the IDB_VARIANT case taken (0 = the
  * default dispatch; the variants exist for f32 rows only)}; all zeros when the last call launched no kernel.  lane = 0xFFFFFFFF: the lane the last call on this index used. */
 IDB_API idb_status idb_last_search_kernel(idb_index* index, uint32_t lane, uint32_t* out);
 /* enabled = 1: reserve persisting L2 for the visited tables on `device` (see idb_search_batch_f32).  enabled = 0 (the default):
@@ -316,7 +326,8 @@ IDB_API idb_status idb_index_load_ex(const char* path, uint32_t dim, uint32_t M,
 /* Same, stored as `storage` (IDB_STORAGE_*); idb_index_load_ex = IDB_STORAGE_F32.  The file always holds f32 rows (a bf16, fp16 or
  * q8 index saves its rows widened or dequantised, exactly), so saving an index and loading it with its own storage gives back the
  * same rows (q8: the same codes and headers).  Unknown storage: IDB_ERR_INVALID_ARG; IDB_STORAGE_F16 and a row value that rounds to
- * infinity in fp16, or IDB_STORAGE_Q8 and a row q8 refuses: IDB_ERR_INVALID_ARG. */
+ * infinity in fp16, or IDB_STORAGE_Q8 and a row q8 refuses, or IDB_STORAGE_BIN and a row element other than 0 or 1:
+ * IDB_ERR_INVALID_ARG; IDB_STORAGE_BIN with IDB_METRIC_COSINE: IDB_ERR_UNSUPPORTED. */
 IDB_API idb_status idb_index_load_storage(const char* path, uint32_t dim, uint32_t M, uint32_t metric, uint32_t storage, int32_t device,
                                           idb_index** out_index, uint64_t* out_values_offset);
 

@@ -738,6 +738,7 @@ idb_status adopt_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M
         if (n_upper && (!upper || !upper_n)) return fail(IDB_ERR_INVALID_ARG, "upper/upper_n is null");
         if (!storage_known(storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
         if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
+        if (idb_status s = check_storage_metric(storage, metric); s != IDB_OK) return s;
         if (metric == IDB_METRIC_COSINE) {
             // Adopted rows are stored as given (normalising is not idempotent bit for bit), so they must already be unit rows; the
             // tolerance lets bf16- and fp16-rounded and q8-quantised unit rows through.
@@ -763,7 +764,7 @@ idb_status adopt_graph(const float* points, uint64_t n, uint32_t dim, uint32_t M
         return s;
     }();
     if (st == IDB_ERR_INVALID_ARG && from_file) st = IDB_ERR_FORMAT;
-    if (st == IDB_OK)  // the rows as given; fp16 / q8 rows beyond the storage's range are refused, named by their row in the call
+    if (st == IDB_OK)  // the rows as given; fp16 / q8 / bin rows beyond the storage's range are refused, named by their row in the call
         st = ix->put_rows(0, n, nullptr, [&](float* dst) { return ix->copy_rows_in(dst, points, n); });
     if (st == IDB_OK) st = ix->build_codes();
     if (st != IDB_OK) {

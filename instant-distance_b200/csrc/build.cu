@@ -400,8 +400,8 @@ idb_status build_index(Index* ix, const float* rows, uint64_t n, uint32_t dim, c
 // Construction::insert(new, 0, layers) (core:437-528) for PointIds [n0, n0 + m), in the build's layer-0 batch schedule from g0 = n0
 // (also when the index has no upper layer, where the build inserts sequentially).  The caller holds the index exclusively and has
 // checked the arguments.  Rows: m x dim host floats, stored as the build stores them (zero padded, normalised for a cosine index,
-// then narrowed for a bf16 or fp16 one or quantised for a q8 one; fp16 / q8 rows beyond the storage's range are refused before
-// the index's rows or graph change).  global_ids: appended to the id map when the index has one.
+// then narrowed for a bf16 or fp16 one, quantised for a q8 one or packed for a bin one; fp16 / q8 / bin rows beyond the storage's
+// range are refused before the index's rows or graph change).  global_ids: appended to the id map when the index has one.
 idb_status insert_index(Index* ix, const float* rows, uint64_t m, const idb_params& p, const uint32_t* global_ids, uint32_t* out_ids) {
     const uint64_t n0 = ix->n, n1 = n0 + m;
     if (out_ids)
@@ -483,6 +483,7 @@ extern "C" idb_status idb_build_ex(const float* rows, uint64_t n, uint32_t dim, 
     if (dim > 10240) return fail(IDB_ERR_UNSUPPORTED, "dim %u > 10240 is not supported (the owner row of a long-row traversal lives in shared memory)", dim);
     if (!(params->ml > 0.0f) || params->ml >= 1.0f) return fail(IDB_ERR_INVALID_ARG, "ml must be in (0, 1)");
     if (!storage_known(params->storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", params->storage);
+    if (idb_status s = check_storage_metric(params->storage, metric); s != IDB_OK) return s;
     if (params->heuristic && params->extend_candidates) return fail(IDB_ERR_UNSUPPORTED, "%s", kNoExtendCandidates);
     auto* ix = new (std::nothrow) Index();
     if (!ix) return fail(IDB_ERR_OOM, "host allocation failed");

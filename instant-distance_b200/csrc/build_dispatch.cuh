@@ -59,9 +59,17 @@ cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStre
     }
     return cudaErrorInvalidValue;
 }
+// The construction cells of bin rows (DESIGN §3d): declared here and defined in bin_cells.cuh, which only build_bin_chN.cu includes,
+// so that they compile in translation units of their own, in parallel with build_chN.cu's cells of the other row types.
+template <int CH, int B, int NB>
+cudaError_t build_dispatch_bin(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st);
 template <int CH, int B, int NB>
 cudaError_t build_dispatch(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    return with_row_type(a.g.row_type, [&](auto rt) { return build_dispatch_rt<CH, B, NB, decltype(rt)>(a, l, st); });
+    return with_row_type(a.g.row_type, [&](auto rt) {
+        using RT = decltype(rt);
+        if constexpr (RT::kType == kRowBin) return build_dispatch_bin<CH, B, NB>(a, l, st);
+        else return build_dispatch_rt<CH, B, NB, RT>(a, l, st);
+    });
 }
 
 // K2's ladder, for other kernels built on select_heuristic_warp (remove.cu): f(CH, NB) as integral constants, with the (CH, NB) that

@@ -65,7 +65,7 @@ __device__ __forceinline__ uint32_t select_heuristic_warp(const GraphView& g, co
     bool cok[CH > 0 ? CH : 1];
 #pragma unroll
     for (int j = 0; j < (CH > 0 ? CH : 1); ++j) cok[j] = (uint32_t)(lane + 32 * j) < g.nchunks;
-    const uint32_t row_bytes = g.nchunks * RT::kChunkBytes;   // global rows (f32, bf16, fp16 or q8)
+    const uint32_t row_bytes = g.nchunks * RT::kChunkBytes;   // global rows (f32, bf16, fp16, q8 or bin)
     const uint32_t srow_bytes = g.nchunks * 16u;               // staged rows are always widened float4
     const char* gbase = g.points + lane * RT::kChunkBytes;
     const char* sbase = reinterpret_cast<const char*>(kept_vecs) + lane * 16;

@@ -35,13 +35,13 @@ constexpr uint32_t kFullMask = 0xFFFFFFFFu;
 enum OptFlags : uint32_t { kOptPrefetchVectors = 1u, kOptPrefetchRows = 2u, kOptPrefetchNextRow = 8u };
 
 // How an index stores its rows; the values are the ABI's IDB_STORAGE_* (internal.cuh checks that).
-enum RowType : uint32_t { kRowF32 = 0, kRowBF16 = 1, kRowF16 = 2, kRowQ8 = 4 };
+enum RowType : uint32_t { kRowF32 = 0, kRowBF16 = 1, kRowF16 = 2, kRowQ8 = 4, kRowBin = 8 };
 
 enum QueryStatus : uint32_t { kQueryOk = 0, kQueryVisitedOverflow = 1, kQueryTieOverflow = 2 };
 
 struct GraphView {
     const char* points;          // n rows of nchunks 4-element chunks (dim rounded up to 4, zero padded); f32 (16 B/chunk), bf16 or fp16
-                                 // (8 B/chunk), q8 (4 B/chunk: one code byte per element)
+                                 // (8 B/chunk), q8 (4 B/chunk: one code byte per element), bin (1 B/chunk: one bit per element)
     uint32_t nchunks;            // 4-element chunks per row
     const uint32_t* zero;        // n x 2M
     const uint32_t* const* upper;  // device array: upper[l-1] = n_l x M
@@ -159,12 +159,28 @@ struct RowQ8 {
     }
     static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
 };
+// bin (DESIGN §3d): 0/1 elements, one byte per chunk (bit k of byte c = element 4c+k, high nibble zero), so a warp's 32 chunks are
+// 32 contiguous bytes.  Each bit widens to exactly 0.f or 1.f, and the zero padding to 0.f.
+struct RowBin {
+    static constexpr uint32_t kType = kRowBin;
+    static constexpr uint32_t kChunkBytes = 1;
+    using Raw = uint32_t;
+    using Hdr = NoHdr;
+    static __device__ __forceinline__ Hdr hdr(const GraphView&, uint32_t) { return Hdr(); }
+    static __device__ __forceinline__ Raw ld_raw(const char* p) { return __ldg(reinterpret_cast<const unsigned char*>(p)); }
+    static __device__ __forceinline__ Raw zero() { return 0u; }
+    static __device__ __forceinline__ float4 widen(Raw u, Hdr) {
+        return make_float4((float)(u & 1u), (float)((u >> 1) & 1u), (float)((u >> 2) & 1u), (float)((u >> 3) & 1u));
+    }
+    static __device__ __forceinline__ float4 ld(const char* p, Hdr h) { return widen(ld_raw(p), h); }
+};
 // f(RT()) for the row type `row_type` of an index: the one place a run-time row type becomes a template argument.
 template <class F>
 auto with_row_type(uint32_t row_type, F&& f) {
     if (row_type == kRowBF16) return f(RowBF16());
     if (row_type == kRowF16) return f(RowF16());
     if (row_type == kRowQ8) return f(RowQ8());
+    if (row_type == kRowBin) return f(RowBin());
     return f(RowF32());
 }
 // Chunk c of a row, widened.  The zero padding of f32 / bf16 / fp16 rows, and the zero Raw loaders put in place of chunks past the
@@ -1186,7 +1202,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, WarpState& s, c
 #ifdef IDB_K1_PHASES
     k1_phase_begin(s);
 #endif
-    constexpr bool kScreen = SCREEN && CH > 0 && !kLive && !TMA && RT::kType != kRowQ8;  // (q8: no table, DESIGN §3c)
+    constexpr bool kScreen = SCREEN && CH > 0 && !kLive && !TMA && RT::kType != kRowQ8 && RT::kType != kRowBin;  // (no table, DESIGN §3c, §3d)
     ScreenQuery<kScreen ? CH : 1> sq;
     if constexpr (kScreen) {
         if (g.codes) screen_query<CH>(sq, g, q.r, lane);

@@ -206,16 +206,17 @@ struct Lane {
 // The stored rows as the export, the save and the screening table read them (Index::stored, rows.cu); K1, the build and the exact scan
 // read them through the row traits of hnsw_device.cuh instead.
 struct StoredRows {
-    const void* rows;      // cap x stride elements of `type`
+    const void* rows;      // cap x stride elements of `type` (bin: cap x stride / 4 bytes)
     const float2* hdr;     // q8 row headers {o, s}
     uint32_t type, stride, dim;
 };
 // Element e (< stride) of stored row r, exactly as f32: bf16 by the 16-bit shift; fp16 by cvt.f32.f16, except that a NaN keeps its
 // sign and payload (cvt.f32.f16 would return the canonical NaN), so an export or a save gives back the f32 value of every stored
-// bit pattern; q8 as fmaf(c, s, o), and 0 past dim.
+// bit pattern; q8 as fmaf(c, s, o), and 0 past dim; bin as bit e % 4 of byte e / 4 (0 in the padding).
 __device__ __forceinline__ float stored_elem(const StoredRows& s, uint64_t r, uint32_t e) {
     const size_t i = r * s.stride + e;
     if (s.type == kRowF32) return static_cast<const float*>(s.rows)[i];
+    if (s.type == kRowBin) return (float)((static_cast<const uint8_t*>(s.rows)[r * (s.stride / 4) + e / 4] >> (e & 3u)) & 1u);
     if (s.type == kRowQ8) {
         const float2 h = s.hdr[r];
         return e < s.dim ? __fmaf_rn((float)static_cast<const uint8_t*>(s.rows)[i], h.y, h.x) : 0.f;
@@ -258,7 +259,7 @@ struct Index {
     std::atomic<uint64_t> n{0};                // written by an insert while other threads may read it (searches take a lane first)
     uint64_t cap = 0;                          // rows allocated for points, zero and the id map (>= n; grows by doubling on insert)
     uint32_t dim = 0, nchunks = 0, M = 32, ef_search = 100;
-    void* d_rows = nullptr;                    // cap x nchunks*4 elements of row_type (PointId order): f32, bf16 / fp16, or q8 codes
+    void* d_rows = nullptr;                    // cap x nchunks*4 elements of row_type (PointId order): f32, bf16 / fp16, q8 codes or bin bits
     float2* d_hdr = nullptr;                   // cap q8 row headers {o, s} (DESIGN §3c), else null
     uint32_t row_type = kRowF32;               // RowType = the IDB_STORAGE_* the rows are stored as; set when the index is created
     uint32_t metric = kMetricL2Sq;             // kMetricCosine: the rows are canonically normalised, and so is every query (DESIGN §3a)
@@ -405,10 +406,13 @@ struct HostCopy {
 idb_status copy_to_host(Lane& ln, const HostCopy* parts, int n_parts, const std::function<cudaError_t()>& also = nullptr);
 
 cudaError_t fill_u32(uint32_t* p, size_t n, uint32_t v, cudaStream_t st);
-static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16 && kRowQ8 == IDB_STORAGE_Q8,
+static_assert(kRowF32 == IDB_STORAGE_F32 && kRowBF16 == IDB_STORAGE_BF16 && kRowF16 == IDB_STORAGE_F16 && kRowQ8 == IDB_STORAGE_Q8 &&
+                  kRowBin == IDB_STORAGE_BIN,
               "RowType mirrors IDB_STORAGE_*");
-// The storage values an index accepts (3 is not one of them).
-inline bool storage_known(uint32_t s) { return s <= IDB_STORAGE_F16 || s == IDB_STORAGE_Q8; }
+// The storage values an index accepts (3 and 5..7 are not among them).
+inline bool storage_known(uint32_t s) { return s <= IDB_STORAGE_F16 || s == IDB_STORAGE_Q8 || s == IDB_STORAGE_BIN; }
+// bin rows take the squared L2 only (DESIGN §3d: normalised rows are not 0/1): IDB_ERR_UNSUPPORTED for cosine, else IDB_OK.
+idb_status check_storage_metric(uint32_t storage, uint32_t metric);
 // normalize_rows_kernel: dst[r] (nchunks * 4 floats, zero padded) = the canonical normalisation of src[r] (src_stride floats per row,
 // dim used, any alignment), one warp per row.  dst may equal src when src_stride == nchunks * 4.
 cudaError_t normalize_rows(const float* src, uint64_t src_stride, float* dst, uint64_t n, uint32_t dim, uint32_t nchunks, int num_sms,

@@ -83,6 +83,7 @@ idb_status idb_index_load_storage(const char* path, uint32_t dim, uint32_t M, ui
     if (dim == 0 || M < 2 || M > 64) return fail(IDB_ERR_INVALID_ARG, "dim/M invalid");
     if (metric != IDB_METRIC_L2SQ && metric != IDB_METRIC_COSINE) return fail(IDB_ERR_INVALID_ARG, "unknown metric %u", metric);
     if (!storage_known(storage)) return fail(IDB_ERR_INVALID_ARG, "unknown storage %u", storage);
+    if (idb_status s = check_storage_metric(storage, metric); s != IDB_OK) return s;
     File in;
     in.f = std::fopen(path, "rb");
     if (!in.f) return fail(IDB_ERR_IO, "cannot open %s", path);

@@ -219,9 +219,10 @@ __global__ void drop_removed_kernel(const uint32_t* removed, uint64_t n, uint32_
         if (is_removed(removed, (uint32_t)x)) new_ids[x] = kInvalid;
 }
 
-// Row x of the store (wpr u32 words: the raw stored row, any storage), its q8 header and its id-map entry -> position new_ids[x].
-__global__ void compact_rows_kernel(const uint32_t* new_ids, uint64_t n, uint32_t wpr, const uint32_t* rows, uint32_t* rows_out,
-                                    const float2* hdr, float2* hdr_out, const uint32_t* id_map, uint32_t* id_map_out) {
+// Row x of the store (wpr words W: the raw stored row, any storage), its q8 header and its id-map entry -> position new_ids[x].
+template <class W>
+__device__ __forceinline__ void compact_rows(const uint32_t* new_ids, uint64_t n, uint32_t wpr, const W* rows, W* rows_out,
+                                             const float2* hdr, float2* hdr_out, const uint32_t* id_map, uint32_t* id_map_out) {
     const uint64_t total = n * wpr;
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t x = i / wpr;
@@ -234,6 +235,15 @@ __global__ void compact_rows_kernel(const uint32_t* new_ids, uint64_t n, uint32_
             if (id_map) id_map_out[y] = id_map[x];
         }
     }
+}
+// Rows that are a whole number of u32 words move as words; bin rows (nchunks bytes, DESIGN §3d) in general are not, and move as bytes.
+__global__ void compact_rows_kernel(const uint32_t* new_ids, uint64_t n, uint32_t wpr, const uint32_t* rows, uint32_t* rows_out,
+                                    const float2* hdr, float2* hdr_out, const uint32_t* id_map, uint32_t* id_map_out) {
+    compact_rows(new_ids, n, wpr, rows, rows_out, hdr, hdr_out, id_map, id_map_out);
+}
+__global__ void compact_rows_kernel(const uint32_t* new_ids, uint64_t n, uint32_t bpr, const uint8_t* rows, uint8_t* rows_out,
+                                    const float2* hdr, float2* hdr_out, const uint32_t* id_map, uint32_t* id_map_out) {
+    compact_rows(new_ids, n, bpr, rows, rows_out, hdr, hdr_out, id_map, id_map_out);
 }
 
 // Adjacency rows [0, n_rows) of `width` entries -> position new_ids[x], every entry relabelled (INVALID stays INVALID).
@@ -338,8 +348,12 @@ idb_status remove_index(Index* ix, const uint32_t* pids, uint64_t m, const idb_p
     drop_removed_kernel<<<blocks, 256, 0, st>>>(b.removed, n, b.new_ids);
     CUDA_TRY(cudaGetLastError());
     if (n1 == 0) CUDA_TRY(fill_u32(next.zero, 2 * (size_t)M, kInvalid, st));  // the one row of an empty store
-    compact_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, (uint32_t)(ix->row_bytes() / 4), static_cast<const uint32_t*>(ix->d_rows),
-                                                static_cast<uint32_t*>(b.rows), ix->d_hdr, b.hdr, ix->d_id_map, b.id_map);
+    if (ix->row_bytes() % 4 == 0)
+        compact_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, (uint32_t)(ix->row_bytes() / 4), static_cast<const uint32_t*>(ix->d_rows),
+                                                    static_cast<uint32_t*>(b.rows), ix->d_hdr, b.hdr, ix->d_id_map, b.id_map);
+    else
+        compact_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, (uint32_t)ix->row_bytes(), static_cast<const uint8_t*>(ix->d_rows),
+                                                    static_cast<uint8_t*>(b.rows), ix->d_hdr, b.hdr, ix->d_id_map, b.id_map);
     CUDA_TRY(cudaGetLastError());
     relabel_rows_kernel<<<blocks, 256, 0, st>>>(b.new_ids, n, 2 * M, ix->graph.zero, next.zero);
     CUDA_TRY(cudaGetLastError());

@@ -1,5 +1,5 @@
-// rows.cu — an index's row storage (DESIGN §2, §3b, §3c): the one buffer of stored rows, the one way rows go in (staged as padded
-// f32, checked against the storage's range, then narrowed or quantised into the store) and the one way they come out (widened
+// rows.cu — an index's row storage (DESIGN §2, §3b, §3c, §3d): the one buffer of stored rows, the one way rows go in (staged as
+// padded f32, checked against the storage's range, then narrowed, quantised or packed into the store) and the one way they come out (widened
 // exactly).  The only host code that branches on the storage type; the kernels read the rows through the row traits of
 // hnsw_device.cuh.
 #include <algorithm>
@@ -11,11 +11,14 @@ namespace idb {
 
 namespace {
 
-size_t elem_bytes(uint32_t row_type) { return row_type == kRowF32 ? 4 : row_type == kRowQ8 ? 1 : 2; }
+// Bytes per stored 4-element chunk (RT::kChunkBytes of the row trait): a bin chunk is a quarter of a q8 one, so there is no per-element size.
+size_t chunk_bytes(uint32_t row_type) {
+    return row_type == kRowF32 ? 16 : row_type == kRowQ8 ? 4 : row_type == kRowBin ? 1 : 8;
+}
 
 // The store of `rows` rows of the index's storage, and q8's headers beside it.
 cudaError_t alloc_store(const Index& ix, uint64_t rows, void** pts, float2** hdr) {
-    cudaError_t e = cudaMalloc(pts, rows * (size_t)ix.nchunks * 4 * elem_bytes(ix.row_type));
+    cudaError_t e = cudaMalloc(pts, rows * ix.row_bytes());
     if (e == cudaSuccess && ix.row_type == kRowQ8) e = cudaMalloc(hdr, rows * sizeof(float2));
     return e;
 }
@@ -116,6 +119,21 @@ __global__ void check_q8_kernel(const float* rows, uint64_t m, uint32_t stride, 
             if (!q8_fits(rint((double)x[i] * g.scale), g.e) || (!o_ok && x[i] == mn)) atomicMin(first, (unsigned long long)(r * stride + i));
     }
 }
+// bin rows (DESIGN §3d): the smallest flat index of an element other than +0.0, -0.0 or 1.0 (NaN, +-inf and subnormals included).
+__global__ void check_bin_kernel(const float* src, size_t n, unsigned long long* first) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t b = __float_as_uint(src[i]);
+        if ((b & 0x7fffffffu) != 0u && b != 0x3f800000u) atomicMin(first, (unsigned long long)i);
+    }
+}
+// Checked 0/1 rows (nchunks * 4 f32 each, so chunk i of the matrix is src[4i, 4i + 4)) -> one byte per chunk: bit k = element 4i+k.
+__global__ void pack_bin_kernel(const float* src, uint8_t* dst, size_t nbytes) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nbytes; i += (size_t)gridDim.x * blockDim.x) {
+        const float4 x = reinterpret_cast<const float4*>(src)[i];
+        dst[i] = (uint8_t)((x.x == 1.f ? 1u : 0u) | (x.y == 1.f ? 2u : 0u) | (x.z == 1.f ? 4u : 0u) | (x.w == 1.f ? 8u : 0u));
+    }
+}
+
 // Codes (stride bytes per row, padding codes 0) and headers of m checked rows.  One warp per row.
 __global__ void quantize_q8_kernel(const float* rows, uint64_t m, uint32_t stride, uint32_t dim, uint8_t* codes, float2* hdr) {
     const int lane = threadIdx.x & 31;
@@ -139,10 +157,11 @@ __global__ void widen_rows_kernel(const StoredRows s, uint64_t r0, uint64_t m, f
 }
 
 // The storage's refusal of m staged rows (nchunks * 4 f32 each, on the device): fp16 refuses a finite element that rounds to +-infinity
-// (|x| >= 65520); q8 a NaN or infinite element, or a row whose header or a dequantised element would overflow f32.  IDB_ERR_INVALID_ARG
+// (|x| >= 65520); q8 a NaN or infinite element, or a row whose header or a dequantised element would overflow f32; bin an element other
+// than +-0 or 1.  IDB_ERR_INVALID_ARG
 // names the first such element and its row, input_row[r] when given, else r.  IDB_OK for the other storages.
 idb_status check_rows(const Index& ix, const float* staged, uint64_t m, const uint32_t* input_row) {
-    if (ix.row_type != kRowF16 && ix.row_type != kRowQ8) return IDB_OK;
+    if (ix.row_type != kRowF16 && ix.row_type != kRowQ8 && ix.row_type != kRowBin) return IDB_OK;
     const size_t stride = (size_t)ix.nchunks * 4;
     unsigned long long* d_first = nullptr;
     unsigned long long first = ~0ull;
@@ -150,6 +169,7 @@ idb_status check_rows(const Index& ix, const float* staged, uint64_t m, const ui
     cudaError_t e = cudaMemcpyAsync(d_first, &first, 8, cudaMemcpyHostToDevice, ix.stream);
     if (e == cudaSuccess) {
         if (ix.row_type == kRowF16) f16_overflow_kernel<<<ix.num_sms * 8, 256, 0, ix.stream>>>(staged, m * stride, d_first);
+        else if (ix.row_type == kRowBin) check_bin_kernel<<<ix.num_sms * 8, 256, 0, ix.stream>>>(staged, m * stride, d_first);
         else check_q8_kernel<<<ix.num_sms * 8, 256, 0, ix.stream>>>(staged, m, (uint32_t)stride, ix.dim, d_first);
         e = cudaGetLastError();
     }
@@ -164,6 +184,8 @@ idb_status check_rows(const Index& ix, const float* staged, uint64_t m, const ui
     if (ix.row_type == kRowF16)
         return fail(IDB_ERR_INVALID_ARG, "fp16 storage: row %llu, element %llu is %g, which rounds to infinity in fp16 (|x| >= 65520)", r,
                     i, (double)x);
+    if (ix.row_type == kRowBin)
+        return fail(IDB_ERR_INVALID_ARG, "bin storage: row %llu, element %llu is %g; bin rows must be 0 or 1", r, i, (double)x);
     if (!std::isfinite(x))
         return fail(IDB_ERR_INVALID_ARG, "q8 storage: row %llu, element %llu is %g; q8 rows must be finite", r, i, (double)x);
     return fail(IDB_ERR_INVALID_ARG, "q8 storage: row %llu, element %llu (%g): the row's dequantised values would overflow f32", r, i,
@@ -171,6 +193,12 @@ idb_status check_rows(const Index& ix, const float* staged, uint64_t m, const ui
 }
 
 }  // namespace
+
+idb_status check_storage_metric(uint32_t storage, uint32_t metric) {
+    if (storage == IDB_STORAGE_BIN && metric == IDB_METRIC_COSINE)
+        return fail(IDB_ERR_UNSUPPORTED, "bin storage takes the squared L2 only: normalised rows are not 0/1");
+    return IDB_OK;
+}
 
 StoredRows Index::stored() const { return StoredRows{d_rows, d_hdr, row_type, nchunks * 4, dim}; }
 
@@ -189,8 +217,10 @@ idb_status Index::put_rows(uint64_t r0, uint64_t m, const uint32_t* input_row, c
     const idb_status s = e == cudaSuccess ? check_rows(*this, staged, m, input_row) : IDB_OK;
     if (s == IDB_OK && e == cudaSuccess && !d_rows) e = alloc_store(*this, cap, &d_rows, &d_hdr);
     if (s == IDB_OK && e == cudaSuccess) {
-        char* dst = static_cast<char*>(d_rows) + r0 * stride * elem_bytes(row_type);
-        if (row_type == kRowQ8)  // normalised first (a cosine index), then quantised
+        char* dst = static_cast<char*>(d_rows) + r0 * row_bytes();
+        if (row_type == kRowBin)
+            pack_bin_kernel<<<num_sms * 8, 256, 0, stream>>>(staged, reinterpret_cast<uint8_t*>(dst), m * nchunks);
+        else if (row_type == kRowQ8)  // normalised first (a cosine index), then quantised
             quantize_q8_kernel<<<num_sms * 8, 256, 0, stream>>>(staged, m, (uint32_t)stride, dim, reinterpret_cast<uint8_t*>(dst), d_hdr + r0);
         else if (row_type == kRowF16)  // normalised first, then rounded
             narrow_f16_kernel<<<num_sms * 8, 256, 0, stream>>>(staged, reinterpret_cast<uint16_t*>(dst), m * stride);
@@ -204,7 +234,7 @@ idb_status Index::put_rows(uint64_t r0, uint64_t m, const uint32_t* input_row, c
     return s;
 }
 
-size_t Index::row_bytes() const { return (size_t)nchunks * 4 * elem_bytes(row_type); }
+size_t Index::row_bytes() const { return (size_t)nchunks * chunk_bytes(row_type); }
 
 cudaError_t Index::alloc_rows(uint64_t rows, void** pts, float2** hdr) const { return alloc_store(*this, rows, pts, hdr); }
 
@@ -219,7 +249,7 @@ cudaError_t Index::copy_rows_in(float* dst, const float* src, uint64_t m) const 
 idb_status Index::reserve_rows(uint64_t rows) {
     if (rows <= cap) return IDB_OK;
     const uint64_t want = std::max<uint64_t>(rows, 2 * cap);
-    const size_t row_bytes = (size_t)nchunks * 4 * elem_bytes(row_type), width = 2 * (size_t)M;
+    const size_t bytes = row_bytes(), width = 2 * (size_t)M;
     void* pts = nullptr;
     float2* hdr = nullptr;
     uint32_t* zero = nullptr;  // the one adjacency layer allocated outside graph.cu: it grows with the rows, all or nothing
@@ -228,7 +258,7 @@ idb_status Index::reserve_rows(uint64_t rows) {
     if (e == cudaSuccess) e = cudaMalloc(&zero, want * width * 4);
     if (e == cudaSuccess && d_id_map) e = cudaMalloc(&id_map, want * 4);
     if (e == cudaSuccess && n) {
-        e = cudaMemcpyAsync(pts, d_rows, n * row_bytes, cudaMemcpyDeviceToDevice, stream);
+        e = cudaMemcpyAsync(pts, d_rows, n * bytes, cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess && hdr) e = cudaMemcpyAsync(hdr, d_hdr, n * sizeof(float2), cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(zero, graph.zero, n * width * 4, cudaMemcpyDeviceToDevice, stream);
         if (e == cudaSuccess && d_id_map) e = cudaMemcpyAsync(id_map, d_id_map, n * 4, cudaMemcpyDeviceToDevice, stream);

@@ -149,7 +149,7 @@ cudaError_t launch_screen_bound(const GraphView& g, const float4* q, const uint3
     const unsigned grid = (unsigned)((npairs + 7) / 8);
     with_row_type(g.row_type, [&](auto rt) {
         using RT = decltype(rt);
-        if constexpr (RT::kType != kRowQ8) screen_bound_kernel<CH, RT><<<grid, 256, 0, st>>>(g, q, pairs, npairs, ob, od);  // (no q8 table)
+        if constexpr (RT::kType != kRowQ8 && RT::kType != kRowBin) screen_bound_kernel<CH, RT><<<grid, 256, 0, st>>>(g, q, pairs, npairs, ob, od);  // (no table)
     });
     return cudaGetLastError();
 }
@@ -161,7 +161,8 @@ idb_status Index::build_codes() {
     cudaFree(d_cparams);
     d_codes = nullptr;
     d_cparams = nullptr;
-    if (!screen || n == 0 || row_type == kRowQ8) return IDB_OK;  // DESIGN §3c: q8 rows are one byte per element already
+    // DESIGN §3c, §3d: q8 rows are one byte per element already, bin rows a quarter byte
+    if (!screen || n == 0 || row_type == kRowQ8 || row_type == kRowBin) return IDB_OK;
     const uint32_t stride = nchunks * 4, cstride = code_words(nchunks) * 4;
     const StoredRows s = stored();
     const unsigned grid = (unsigned)std::min<uint64_t>((n + 63) / 64, (uint64_t)num_sms * 8);
@@ -220,7 +221,7 @@ extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* quer
                                              float* out_bound, float* out_dist) {
     if (!index || (npairs && (!queries || !pairs || !out_bound || !out_dist))) return fail(IDB_ERR_INVALID_ARG, "null argument");
     Index* ix = reinterpret_cast<Index*>(index);
-    if (!ix->d_codes) return fail(IDB_ERR_UNSUPPORTED, "this index has no screening table (IDB_SCREEN=0, empty, q8 rows, or a non-finite value)");
+    if (!ix->d_codes) return fail(IDB_ERR_UNSUPPORTED, "this index has no screening table (IDB_SCREEN=0, empty, q8 or bin rows, or a non-finite value)");
     const int ch = kernel_ch(ix->nchunks);
     if (ch == 0) return fail(IDB_ERR_UNSUPPORTED, "dim %u: rows of more than 1024 elements are not screened", ix->dim);
     for (uint64_t i = 0; i < npairs; ++i)

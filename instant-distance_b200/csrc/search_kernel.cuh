@@ -201,14 +201,21 @@ cudaError_t dispatch_row_ef_rt(const SearchArgs& a, int row_t, int ef_t, int gri
         return launch_search<CH, ROW_T, EF_T, B, kSearchCtasPerSm, RT, false>(a, grid, st, win);
     });
 }
+// Rows in flight per lane for row type RT, given B for f32 rows: bf16 / fp16 / q8 / bin rows stay packed while in flight (a half or a
+// quarter of the registers per row), so twice the rows, up to 16 (q8 takes the 2-byte rule: it also carries a header per row; bin
+// takes it too, one register per chunk as q8).
+template <int B, class RT>
+constexpr int rows_in_flight() { return RT::kChunkBytes <= 8 && 2 * B <= 16 ? 2 * B : B; }
+// K1's bin-row cells (DESIGN §3d): declared here and defined in bin_cells.cuh, which only search_bin_chN.cu includes, so that they
+// are compiled in translation units of their own, in parallel with search_chN.cu's cells of the other row types.
+template <int CH, int B>
+cudaError_t dispatch_row_ef_bin(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win);
 template <int CH, int B>
 cudaError_t dispatch_row_ef(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    // bf16 / fp16 / q8 rows stay packed while in flight (a half or a quarter of the registers per row): twice the rows in flight per
-    // lane, up to 16 (q8 takes the 2-byte rule: it also carries a header per row)
     return with_row_type(a.g.row_type, [&](auto rt) {
         using RT = decltype(rt);
-        constexpr int BR = RT::kChunkBytes <= 8 && 2 * B <= 16 ? 2 * B : B;
-        return dispatch_row_ef_rt<CH, BR, RT>(a, row_t, ef_t, grid, st, win);
+        if constexpr (RT::kType == kRowBin) return dispatch_row_ef_bin<CH, B>(a, row_t, ef_t, grid, st, win);
+        else return dispatch_row_ef_rt<CH, rows_in_flight<B, RT>(), RT>(a, row_t, ef_t, grid, st, win);
     });
 }
 

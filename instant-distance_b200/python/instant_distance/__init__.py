@@ -18,6 +18,10 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
     §3b: results are those of the f32 index on the rounded points; "f16" refuses values that round to infinity, |x| >= 65520).
   * `Config.storage = "q8"` keeps them as one byte per element on a grid of each point's own (DESIGN.md §3c: results are those of
     the f32 index on the dequantised points; points with a NaN or infinite value, or whose grid would overflow f32, are refused).
+  * `Config.storage = "bin"` keeps 0/1 points at one byte per four elements (DESIGN.md §3d): every point value must be 0.0, -0.0
+    or 1.0 (others are refused), and the metric must be "l2sq".  Queries are any floats; the reported distance is the squared L2 to
+    the 0/1 point, which for 0/1 queries is exactly the Hamming distance.  Packed codes (8 bits per byte) unpack with
+    `np.unpackbits(codes, axis=1).astype(np.float32)`.
     The file holds the points widened to f32, so `Hnsw.load / HnswMap.load(..., storage=)` take the storage too.
 """
 import ctypes as C
@@ -49,7 +53,7 @@ class Config:
         self.seed = random.getrandbits(64)
         self.heuristic = Heuristic()
         self.metric = "l2sq"  # or "cosine"
-        self.storage = "f32"  # or "bf16", "f16", "q8"
+        self.storage = "f32"  # or "bf16", "f16", "q8", "bin"
 
     def _params(self):
         kw = dict(ef_search=self.ef_search, ef_construction=self.ef_construction, ml=self.ml, seed=self.seed, metric=self.metric,

@@ -151,8 +151,9 @@ def ptr(a, t):
     return a.ctypes.data_as(C.POINTER(t))
 
 
-# IDB_STORAGE_*: how an index keeps its rows (2-byte rows are widened exactly to f32; q8 rows are dequantised exactly, DESIGN.md §3c)
-STORAGE = {"f32": 0, "bf16": 1, "f16": 2, "q8": 4}
+# IDB_STORAGE_*: how an index keeps its rows (2-byte rows are widened exactly to f32; q8 rows are dequantised exactly, DESIGN.md §3c;
+# bin rows are 0/1, one byte per four elements, DESIGN.md §3d)
+STORAGE = {"f32": 0, "bf16": 1, "f16": 2, "q8": 4, "bin": 8}
 METRIC = {"l2sq": 0, "cosine": 1}  # IDB_METRIC_*: squared L2, or 1 - cos through canonically normalised rows (DESIGN.md §3a)
 
 
@@ -268,7 +269,7 @@ class Index:
     @classmethod
     def load(cls, path, dim=300, M=32, device=0, metric="l2sq", storage="f32"):
         """Returns (Index, offset of the HnswMap values in the file).  The file records neither the metric nor the storage: it
-        holds f32 rows, stored again as `storage` ("f32", "bf16", "f16" or "q8")."""
+        holds f32 rows, stored again as `storage` ("f32", "bf16", "f16", "q8" or "bin")."""
         h, off = C.c_void_p(), C.c_uint64()
         check(lib().idb_index_load_storage(os.fsencode(path), dim, M, _metric(metric), _storage(storage), device, C.byref(h),
                                            C.byref(off)))
@@ -378,7 +379,7 @@ class Index:
 
     def last_kernel(self, lane=0xFFFFFFFF):
         """The search-kernel instantiation the last call launched, as a dict over KERNEL_FIELDS (all zeros: none launched).
-        The "bf16" field carries the row type, a STORAGE value: 0 f32, 1 bf16, 2 f16, 4 q8."""
+        The "bf16" field carries the row type, a STORAGE value: 0 f32, 1 bf16, 2 f16, 4 q8, 8 bin."""
         out = (C.c_uint32 * 8)()
         check(lib().idb_last_search_kernel(self._h, lane, out))
         return dict(zip(self.KERNEL_FIELDS, (int(v) for v in out)))

@@ -81,11 +81,13 @@ pub const METRIC_COSINE: u32 = 1;
 
 /// How an index stores its rows (include/instant_distance_b200.h IDB_STORAGE_*, the `storage` field of `IdbParams`): f32, rounded
 /// to bf16 / fp16 (half the bytes; fp16 refuses values that round to infinity), or quantised to a per-row 8-bit grid (q8: a quarter
-/// of the bytes plus 8 per row; refuses non-finite rows).  Distances stay fp32 on the exactly widened or dequantised rows.
+/// of the bytes plus 8 per row; refuses non-finite rows), or kept as 0/1 bits (bin: one byte per four elements; refuses any other
+/// value and the cosine metric).  Distances stay fp32 on the exactly widened or dequantised rows.
 pub const STORAGE_F32: u32 = 0;
 pub const STORAGE_BF16: u32 = 1;
 pub const STORAGE_F16: u32 = 2;
 pub const STORAGE_Q8: u32 = 4;
+pub const STORAGE_BIN: u32 = 8;
 
 /// The canonical normalisation the cosine metric applies, evaluated on `device` (rows: n x dim, row-major).
 pub fn normalize(rows: &[f32], dim: usize, device: i32) -> Vec<f32> {
