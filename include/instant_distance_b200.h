@@ -269,6 +269,31 @@ IDB_API idb_status idb_range_search_batch_device_lane(idb_index* index, uint32_t
                                                       float radius, uint64_t capacity, uint64_t* d_out_offsets,
                                                       uint32_t* d_out_ids, float* d_out_dist, uint64_t* out_total);
 
+/* Graph range search (DESIGN.md §9c): the points within `radius` of each query that layer 0 reaches from the query's approximate
+ * nearest neighbours, at a cost that follows the hits rather than the number of points.  The result may miss points the exact range
+ * search finds, but it is a deterministic set:
+ *   seeds: nearest(q) is what idb_search_batch_f32(index, q, 1, ef_search, k = ef) returns (PointIds before the id map), and the
+ *     seeds are its members whose reported distance is <= radius;
+ *   closure: the smallest set H(q) that holds the seeds and, with every point p, every layer-0 neighbour x of p (the entries of p's
+ *     layer-0 row up to its first IDB_INVALID) whose reported distance is <= radius.
+ * H(q) is a subset of the exact range search's result with the same distances, so its hits are a subsequence of that result.  The
+ * radius edges, the order (distance, then PointId; ids through the id map after ordering), the CSR output, `capacity`, the counting
+ * call, IDB_ERR_CAPACITY with out_offsets written, the size limits and the argument errors are those of idb_range_search_batch_f32.
+ * ef_search: 0 = the index's, else 1..1024 (else IDB_ERR_INVALID_ARG).  The seed search is an approximate search and updates the
+ * approximate-search diagnostics as one at the same ef_search would.  A query whose seed search overflowed even its retry pass makes
+ * the call return IDB_ERR_CAPACITY with idb_last_search_failures(index, lane) > 0 (the results of the other queries are written
+ * when the total fits).  The expansion itself never gives up on a query: the queries that overflow its per-query scratch are run
+ * again with scratch for every point (up to 2 GB per call); only a failed allocation is an error (IDB_ERR_OOM).  Takes an idle
+ * submission lane.  nq == 0: IDB_OK, out_offsets[0] = 0 (when given). */
+IDB_API idb_status idb_graph_range_search_batch_f32(idb_index* index, const float* queries, uint64_t nq, uint32_t ef_search, float radius,
+                                                    uint64_t capacity, uint64_t* out_offsets, uint32_t* out_ids, float* out_dist);
+/* Same, device pointers, on submission lane `lane`, with the total in the HOST word *out_total: as idb_range_search_batch_device_lane,
+ * it returns only after the lane has run the call. */
+IDB_API idb_status idb_graph_range_search_batch_device_lane(idb_index* index, uint32_t lane, const float* d_queries, uint64_t nq,
+                                                            uint32_t ef_search, float radius, uint64_t capacity,
+                                                            uint64_t* d_out_offsets, uint32_t* d_out_ids, float* d_out_dist,
+                                                            uint64_t* out_total);
+
 IDB_API uint32_t idb_index_num_lanes(void);
 IDB_API void* idb_index_lane_stream(idb_index* index, uint32_t lane);  /* cudaStream_t of that lane */
 /* Waits for the last call on `lane` and reports how many of its queries failed even in the retry pass (0 = all results valid). */

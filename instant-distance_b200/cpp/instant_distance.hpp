@@ -122,6 +122,25 @@ class Hnsw {
             out.push_back(Item{search.dist_[i], PointId{search.ids_[i]}, &points_[search.ids_[i]]});
         return out;
     }
+    // Not in the reference: the points within `radius` of `point` that layer 0 reaches from its ef_search approximate nearest
+    // neighbours through points within `radius` (idb_graph_range_search_batch_f32, DESIGN.md §9c; ef_search 0 = the index's), nearest
+    // first, ties by lower PointId.  A subset of the exact range search's result, at a cost that follows the hits.
+    std::vector<Item> search_range_graph(const Point& point, float radius, uint32_t ef_search = 0) const {
+        if (!points_.empty() && point.v.size() != points_[0].v.size()) throw Error(IDB_ERR_INVALID_ARG, "query dimension differs from the index");
+        uint64_t offsets[2] = {0, 0};
+        std::vector<uint32_t> ids(1024);
+        std::vector<float> dist(1024);
+        idb_status st = idb_graph_range_search_batch_f32(raw_, point.v.data(), 1, ef_search, radius, ids.size(), offsets, ids.data(), dist.data());
+        if (st == IDB_ERR_CAPACITY && offsets[1] > ids.size()) {  // once more, sized exactly
+            ids.resize(offsets[1]);
+            dist.resize(offsets[1]);
+            st = idb_graph_range_search_batch_f32(raw_, point.v.data(), 1, ef_search, radius, ids.size(), offsets, ids.data(), dist.data());
+        }
+        check(st);
+        std::vector<Item> out;
+        for (uint64_t i = 0; i < offsets[1]; ++i) out.push_back(Item{dist[i], PointId{ids[i]}, &points_[ids[i]]});
+        return out;
+    }
     // #[doc(hidden)] get (lib.rs:394-396)
     std::optional<Item> get(size_t i, const Search& s) const {
         if (i >= s.len_) return std::nullopt;

@@ -353,6 +353,7 @@ idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shar
         if (rc->capacity > 0 && !rc->ids)
             return fail(IDB_ERR_INVALID_ARG, "out_ids is null with capacity %llu", (unsigned long long)rc->capacity);
         if (std::isnan(rc->radius)) return fail(IDB_ERR_INVALID_ARG, "radius is NaN");
+        if (rc->ef_search > kMaxEf) return fail(IDB_ERR_INVALID_ARG, "ef_search %u is not 0 or 1..%u", rc->ef_search, kMaxEf);
         if (rc->device && !rc->out_total) return fail(IDB_ERR_INVALID_ARG, "out_total is null");
         if (rc->capacity > kRangeMaxCapacity || nq >= kRangeMaxCapacity)
             return fail(IDB_ERR_UNSUPPORTED, "the range search takes a capacity of at most %llu and fewer queries (capacity %llu, nq %llu)",
@@ -378,6 +379,7 @@ void Lane::free_all() {
     cudaFree(q); cudaFree(qn); cudaFree(ids); cudaFree(dist); cudaFree(len);
     cudaFree(keys_local); cudaFree(keys_all); cudaFree(shard_ids); cudaFree(exact_keys);
     cudaFree(range_keys); cudaFree(range_qids); cudaFree(range_seg); cudaFree(range_off); cudaFree(range_tmp);
+    cudaFree(gr_seeds); cudaFree(gr_front); cudaFree(gr_vis); cudaFree(gr_ctl); cudaFree(gr_retry);
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (ev_ctrl) cudaEventDestroy(ev_ctrl);
@@ -577,7 +579,7 @@ idb_status Index::normalize_queries(Lane& ln, const float** q, uint64_t nq) {
 }
 
 idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged, uint64_t nq, uint32_t ef_search, uint32_t k,
-                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys) {
+                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys, bool map_ids) {
     CUDA_TRY(cudaSetDevice(ix->device));
     const uint32_t ef = ef_search ? ef_search : ix->ef_search;
     if (ix->n == 0 || ef == 0) {  // empty index (core:359-361) / ef_search = 0: empty result lists
@@ -589,12 +591,12 @@ idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged
         idb_status st = ix->stage_queries(ln, queries, false, nq, &queries);
         if (st != IDB_OK) return st;
     }
-    return ix->enqueue_search(ln, queries, nq, ef, k, d_ids, d_dist, d_len, d_keys);
+    return ix->enqueue_search(ln, queries, nq, ef, k, d_ids, d_dist, d_len, d_keys, map_ids);
 }
 
 // Enqueue one batched search on a lane; all pointers are device pointers (d_queries: see internal.cuh).  The caller holds ln.mu.
 idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids, float* d_dist,
-                                 uint32_t* d_len, uint64_t* out_keys) {
+                                 uint32_t* d_len, uint64_t* out_keys, bool map_ids) {
     if (n) ef = (uint32_t)std::min<uint64_t>(ef, n);  // admission is rank < ef and there are only n distinct ids: same results
     if (ef > 1024) return fail(IDB_ERR_UNSUPPORTED, "ef_search %u > 1024 (on an index of more than 1024 points) is not supported", ef);
     idb_status st = ensure_lane_scratch(ln, nq);
@@ -618,7 +620,7 @@ idb_status Index::enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, 
     a.counters = ln.counters;
     a.variant = variant;
     a.out_keys = out_keys;
-    a.id_map = d_id_map;
+    a.id_map = map_ids ? d_id_map : nullptr;
     a.full_tally = &ln.ctrl->full_fetches;  // K1 and the retry pass both add to it
     std::memset(ln.last_kernel, 0, sizeof(ln.last_kernel));
     a.launched = ln.last_kernel;
@@ -718,6 +720,7 @@ idb_status Index::init_device(int dev) {
     if (const char* e = std::getenv("IDB_VIS_SLOTS")) vis_slots_override = next_pow2((uint64_t)std::max(64, std::atoi(e)));
     if (const char* e = std::getenv("IDB_SCREEN")) screen = std::atoi(e) != 0;
     if (const char* e = std::getenv("IDB_EXACT_SCRATCH_KEYS")) exact_scratch_keys = (uint64_t)std::max(1LL, std::atoll(e));
+    if (const char* e = std::getenv("IDB_GRAPH_RANGE_SCRATCH")) graph_range_scratch = (uint32_t)std::min(1 << 20, std::max(1, std::atoi(e)));
     return IDB_OK;
 }
 

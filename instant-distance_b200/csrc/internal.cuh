@@ -183,6 +183,13 @@ struct Lane {
     uint64_t* range_seg = nullptr;  size_t range_seg_cap = 0;
     uint64_t* range_off = nullptr;  size_t range_off_cap = 0;
     uint64_t* range_tmp = nullptr;  size_t range_tmp_cap = 0;
+    // graph range search (graph_range.cu): the seed search's keys, the main pass's per-warp frontiers and visited tables, its
+    // control words and overflow list, and the retry pass's per-warp frontiers and bitmaps
+    uint64_t* gr_seeds = nullptr;   size_t gr_seeds_cap = 0;
+    uint64_t* gr_front = nullptr;   size_t gr_front_cap = 0;
+    uint32_t* gr_vis = nullptr;     size_t gr_vis_cap = 0;
+    uint32_t* gr_ctl = nullptr;     size_t gr_ctl_cap = 0;
+    uint64_t* gr_retry = nullptr;   size_t gr_retry_cap = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // host API: results land here first when the caller's output buffers are pageable (see read_back in api.cu)
     unsigned char* h_out = nullptr; size_t h_out_cap = 0;   // pinned
@@ -285,6 +292,7 @@ struct Index {
     int vis_tier = -1;            // IDB_VIS_TIER: -1 auto (b16 when exact for this n, else bitmap / hash), 0 hash, 1 bitmap, 2 b16
     int variant = 0;              // IDB_VARIANT: alternative (rows in flight, CTAs/SM) instantiations of K1
     uint64_t exact_scratch_keys = 0;  // IDB_EXACT_SCRATCH_KEYS (tests): keys of an exact call's list scratch per query chunk (0 = default)
+    uint32_t graph_range_scratch = 0; // IDB_GRAPH_RANGE_SCRATCH (tests): hits per query the graph range search's main pass holds (0 = default)
     // Adaptive: when more than 1 in 1000 traversals of a call overflowed the b16 tables (data whose traversals visit more ids than
     // the tables were sized for), later calls with that ef or a larger one use the DRAM-resident atomic flavours instead of paying
     // for the retry pass.  Results are identical either way.
@@ -334,9 +342,9 @@ struct Index {
     idb_status stage_queries(Lane& ln, const float* queries, bool host, uint64_t nq, const float** out);
     // A cosine index normalises the staged rows *q once per call into ln.qn and points *q there; an L2 index reads them as staged.
     idb_status normalize_queries(Lane& ln, const float** q, uint64_t nq);
-    // d_queries: staged rows (stage_queries).
+    // d_queries: staged rows (stage_queries).  map_ids = false: ids and keys carry PointIds even when the index has an id map.
     idb_status enqueue_search(Lane& ln, const float* d_queries, uint64_t nq, uint32_t ef, uint32_t k, uint32_t* d_ids, float* d_dist,
-                              uint32_t* d_len, uint64_t* out_keys);
+                              uint32_t* d_len, uint64_t* out_keys, bool map_ids = true);
     Lane& pick_lane();
     // For the idb_last_search_* queries: under the lane's lock, what the lane's last search left behind — its control block (`ctrl`,
     // once the lane's stream has drained) and its K1 instantiation (`kernel`, 8 words) — each optional, all zero when the lane has
@@ -370,7 +378,7 @@ idb_status require_device(int* count = nullptr);
 // nq = 0 and caps k at kExactMaxK; `lane` (optional) must name a lane, even when nq = 0; `sharded` checks comm before anything else
 // and the list of n_shards handles only when nq > 0 (the others check their one handle first).  nq = 0 passes once the checks that
 // apply to it have, without the device check: there is nothing to do.
-// `range` takes no k; out_ids stands for its offsets, and `rc` carries what else it checks.
+// `range` (the exact and the graph range search) takes no k; out_ids stands for its offsets, and `rc` carries what else it checks.
 enum class Family { approx, exact, sharded, range };
 struct RangeCheck {
     float radius;
@@ -378,7 +386,9 @@ struct RangeCheck {
     const void* ids;
     bool device;                 // the device entry, which reports the total in *out_total
     const uint64_t* out_total;
+    uint32_t ef_search;          // the graph range search's seed search width: 0 (the index's) or 1..kMaxEf; 0 for the exact one
 };
+constexpr uint32_t kMaxEf = 1024;                    // the largest ef_search a search takes
 constexpr uint64_t kRangeMaxCapacity = 0x7fffffffu;  // CUB's sorts and scans take int sizes: capacity <= this, nq + 1 <= this
 idb_status check_search_args(Family f, idb_index* const* shards, uint32_t n_shards, const void* comm, const uint32_t* lane,
                              const void* queries, uint64_t nq, const void* out_ids, uint32_t k, const RangeCheck* rc = nullptr);
@@ -389,7 +399,24 @@ cudaError_t write_empty(cudaStream_t st, uint64_t nq, uint32_t k, uint32_t* ids,
 // One approximate search on a lane (the caller holds ln.mu) of staged queries (`staged`) or of the caller's device queries (dim
 // floats per row, any alignment); empty result lists for an empty index or ef_search = 0.
 idb_status search_on_lane(Index* ix, Lane& ln, const float* queries, bool staged, uint64_t nq, uint32_t ef_search, uint32_t k,
-                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys);
+                          uint32_t* d_ids, float* d_dist, uint32_t* d_len, uint64_t* d_keys, bool map_ids = true);
+
+// Where a range search's collector puts its hits (range.cu): counts[q] (nq, zeroed) = query q's hits; each hit as a (key, query) pair at
+// a position claimed from *total (zeroed), written only below `capacity`.
+struct RangeSink {
+    uint32_t* counts;
+    unsigned long long* total;
+    uint64_t capacity;
+    uint64_t* keys;
+    uint32_t* qids;
+};
+// A range search of nq queries on the lane (the caller holds ln.mu; DESIGN §9b, §9c): collect(sink) enqueues the kernels that append the
+// hits; then the offsets (the exclusive scan of the counts), the total read back, the capacity check (IDB_ERR_CAPACITY, offsets and
+// total written), the gather into each query's segment, the segmented sort by key and the ids (through the id map) and reported
+// distances.  Host call: offsets, ids and dist are the caller's host buffers; device call: device buffers, the total goes to
+// *out_total.  Returns once the lane has run the call.
+idb_status range_on_lane(Index* ix, Lane& ln, bool host, uint64_t nq, uint64_t capacity, uint64_t* offsets, uint32_t* ids, float* dist,
+                         uint64_t* out_total, const std::function<idb_status(const RangeSink&)>& collect);
 
 // The end of a host call on lane ln: copies its results (ln.ids / dist / len, nq x k) to the caller's buffers (each but out_ids
 // optional), reads the control block of each of `ctrl_lanes` whose last call ran K1 into its pinned h_ctrl[1], synchronises the

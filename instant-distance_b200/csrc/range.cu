@@ -136,26 +136,28 @@ unsigned grid_for(const Index* ix, uint64_t items) {
 // CUB's scratch for `bytes` bytes in the lane's buffer.
 cudaError_t ensure_tmp(Lane& ln, size_t bytes) { return ensure_u64(ln.range_tmp, ln.range_tmp_cap, (bytes + 7) / 8); }
 
-// Frees the lane's pair scratch at the end of a call when one large call grew it past kRangeScratchBytes.
+// Frees the lane's pair scratch (and the graph range search's expansion scratch) at the end of a call when one large call grew it past
+// kRangeScratchBytes.
 struct TrimScratch {
     Lane& ln;
     ~TrimScratch() {
-        if (ln.range_keys_cap * 8 + ln.range_qids_cap * 4 + ln.range_seg_cap * 8 + ln.range_tmp_cap * 8 <= kRangeScratchBytes) return;
+        if (ln.range_keys_cap * 8 + ln.range_qids_cap * 4 + ln.range_seg_cap * 8 + ln.range_tmp_cap * 8 + ln.gr_front_cap * 8 +
+                ln.gr_vis_cap * 4 + ln.gr_retry_cap * 8 <=
+            kRangeScratchBytes)
+            return;
         cudaStreamSynchronize(ln.stream);
         cudaFree(ln.range_keys); cudaFree(ln.range_qids); cudaFree(ln.range_seg); cudaFree(ln.range_tmp);
-        ln.range_keys = ln.range_seg = ln.range_tmp = nullptr;
-        ln.range_qids = nullptr;
-        ln.range_keys_cap = ln.range_qids_cap = ln.range_seg_cap = ln.range_tmp_cap = 0;
+        cudaFree(ln.gr_front); cudaFree(ln.gr_vis); cudaFree(ln.gr_retry);
+        ln.range_keys = ln.range_seg = ln.range_tmp = ln.gr_front = ln.gr_retry = nullptr;
+        ln.range_qids = ln.gr_vis = nullptr;
+        ln.range_keys_cap = ln.range_qids_cap = ln.range_seg_cap = ln.range_tmp_cap = ln.gr_front_cap = ln.gr_vis_cap = ln.gr_retry_cap = 0;
     }
 };
 
 }  // namespace
 
-// The range search of nq queries (dim floats per row, any alignment, in host memory when `host`, else on the index's device) on the
-// lane (the caller holds ln.mu).  Host call: offsets, ids and dist are the caller's host buffers; device call: device buffers, and
-// the total goes to *out_total.  Returns once the lane has run the call.
-static idb_status run_range(Index* ix, Lane& ln, const float* queries, bool host, uint64_t nq, float radius, uint64_t capacity,
-                            uint64_t* offsets, uint32_t* ids, float* dist, uint64_t* out_total) {
+idb_status range_on_lane(Index* ix, Lane& ln, bool host, uint64_t nq, uint64_t capacity, uint64_t* offsets, uint32_t* ids, float* dist,
+                         uint64_t* out_total, const std::function<idb_status(const RangeSink&)>& collect) {
     CUDA_TRY(cudaSetDevice(ix->device));
     TrimScratch trim{ln};
     cudaStream_t st = ln.stream;
@@ -170,39 +172,8 @@ static idb_status run_range(Index* ix, Lane& ln, const float* queries, bool host
         CUDA_TRY(ensure_u64(ln.range_keys, ln.range_keys_cap, capacity));
         CUDA_TRY(ensure_u32(ln.range_qids, ln.range_qids_cap, capacity));
     }
-
-    if (ix->n > 0) {
-        const float* qp = nullptr;
-        idb_status s = ix->stage_queries(ln, queries, host, nq, &qp);
-        if (s == IDB_OK) s = ix->normalize_queries(ln, &qp, nq);
-        if (s != IDB_OK) return s;
-        const RangeChoice rc = pick_range(ix->nchunks, ix->row_type);
-        ScanLaunch sl;
-        s = scan_launch(ix, rc.fn, &sl);
-        if (s != IDB_OK) return s;
-        // Slices: enough CTAs for about four waves of the device, at least kScanMinSliceRows rows each.
-        const uint64_t q_per_cta = (uint64_t)sl.wpc * rc.qw;
-        const uint64_t want_ctas = 4ull * std::max(1, sl.occ) * ix->num_sms;
-        const uint64_t q_ctas = (nq + q_per_cta - 1) / q_per_cta;
-        uint64_t S = (want_ctas + q_ctas - 1) / q_ctas;
-        S = std::min<uint64_t>(S, (ix->n + kScanMinSliceRows - 1) / kScanMinSliceRows);
-        S = std::max<uint64_t>(S, 1);
-        RangeArgs a;
-        std::memset(&a, 0, sizeof(a));
-        a.g = ix->view();
-        a.queries = reinterpret_cast<const float4*>(qp);
-        a.nq = nq;
-        a.slice_rows = (ix->n + S - 1) / S;
-        a.radius = radius;
-        a.metric = ix->metric;
-        a.counts = counts;
-        a.total = d_total;
-        a.capacity = capacity;
-        a.keys = ln.range_keys;
-        a.qids = ln.range_qids;
-        rc.fn<<<dim3((unsigned)q_ctas, (unsigned)S), sl.wpc * 32, sl.smem, st>>>(a);
-        CUDA_TRY(cudaGetLastError());
-    }
+    idb_status s = collect(RangeSink{counts, d_total, capacity, ln.range_keys, ln.range_qids});
+    if (s != IDB_OK) return s;
 
     // offsets = the exclusive scan of the counts; offsets[nq] = the total
     size_t scan_bytes = 0;
@@ -211,7 +182,7 @@ static idb_status run_range(Index* ix, Lane& ln, const float* queries, bool host
     CUDA_TRY(cub::DeviceScan::ExclusiveScan(ln.range_tmp, scan_bytes, counts, d_off, ::cuda::std::plus<>{}, (uint64_t)0, (int)(nq + 1), st));
     uint64_t total = 0;
     const HostCopy hc = host ? HostCopy{offsets, d_off, (nq + 1) * 8} : HostCopy{out_total, d_off + nq, 8};
-    idb_status s = copy_to_host(ln, &hc, 1);
+    s = copy_to_host(ln, &hc, 1);
     if (s != IDB_OK) return s;
     total = host ? offsets[nq] : *out_total;
     if (total > capacity)
@@ -239,6 +210,46 @@ static idb_status run_range(Index* ix, Lane& ln, const float* queries, bool host
     }
     const HostCopy out[2] = {{ids, d_ids, total * 4}, {dist, d_dist, total * 4}};
     return copy_to_host(ln, out, 2);
+}
+
+// The exact range search of nq queries (dim floats per row, any alignment, in host memory when `host`, else on the index's device) on
+// the lane (the caller holds ln.mu): range_scan_kernel over every stored row collects the hits.
+static idb_status run_range(Index* ix, Lane& ln, const float* queries, bool host, uint64_t nq, float radius, uint64_t capacity,
+                            uint64_t* offsets, uint32_t* ids, float* dist, uint64_t* out_total) {
+    return range_on_lane(ix, ln, host, nq, capacity, offsets, ids, dist, out_total, [&](const RangeSink& sink) -> idb_status {
+        if (ix->n == 0) return IDB_OK;
+        const float* qp = nullptr;
+        idb_status s = ix->stage_queries(ln, queries, host, nq, &qp);
+        if (s == IDB_OK) s = ix->normalize_queries(ln, &qp, nq);
+        if (s != IDB_OK) return s;
+        const RangeChoice rc = pick_range(ix->nchunks, ix->row_type);
+        ScanLaunch sl;
+        s = scan_launch(ix, rc.fn, &sl);
+        if (s != IDB_OK) return s;
+        // Slices: enough CTAs for about four waves of the device, at least kScanMinSliceRows rows each.
+        const uint64_t q_per_cta = (uint64_t)sl.wpc * rc.qw;
+        const uint64_t want_ctas = 4ull * std::max(1, sl.occ) * ix->num_sms;
+        const uint64_t q_ctas = (nq + q_per_cta - 1) / q_per_cta;
+        uint64_t S = (want_ctas + q_ctas - 1) / q_ctas;
+        S = std::min<uint64_t>(S, (ix->n + kScanMinSliceRows - 1) / kScanMinSliceRows);
+        S = std::max<uint64_t>(S, 1);
+        RangeArgs a;
+        std::memset(&a, 0, sizeof(a));
+        a.g = ix->view();
+        a.queries = reinterpret_cast<const float4*>(qp);
+        a.nq = nq;
+        a.slice_rows = (ix->n + S - 1) / S;
+        a.radius = radius;
+        a.metric = ix->metric;
+        a.counts = sink.counts;
+        a.total = sink.total;
+        a.capacity = sink.capacity;
+        a.keys = sink.keys;
+        a.qids = sink.qids;
+        rc.fn<<<dim3((unsigned)q_ctas, (unsigned)S), sl.wpc * 32, sl.smem, ln.stream>>>(a);
+        CUDA_TRY(cudaGetLastError());
+        return IDB_OK;
+    });
 }
 
 }  // namespace idb

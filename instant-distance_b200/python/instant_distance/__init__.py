@@ -10,6 +10,8 @@ Everything numeric happens in libinstant_distance_b200.so through the C ABI (no 
     the ground truth to tune `ef_search` against;
   * `Hnsw.search_range / HnswMap.search_range` return every point within a radius of each query (exact, however many there are;
     DESIGN.md §9b), nearest first, as CSR;
+  * `Hnsw.search_range_graph / HnswMap.search_range_graph` return the points within a radius that the graph reaches from each
+    query's approximate nearest neighbours (a subset of search_range's result at a cost that follows the hits; DESIGN.md §9c);
   * `Hnsw.insert / HnswMap.insert` append points to a built or loaded index (layer 0 only, PointIds continue from the current
     count; DESIGN.md §6);
   * `Config.metric = "cosine"` builds an index that reports 1 - cos (points and queries normalised in the canonical order,
@@ -147,6 +149,13 @@ class Hnsw:
         ids [total], distances [total]); query i's neighbours are ids[offsets[i]:offsets[i + 1]], nearest first, ties by PointId."""
         q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
         return self._ix.range_search(q, radius)
+
+    def search_range_graph(self, points, radius, ef_search=None):
+        """The points within `radius` of each query that layer 0 reaches from the query's ef_search nearest neighbours (default: the
+        index's ef_search) through points within `radius` (DESIGN.md §9c): a subset of search_range's result with the same
+        distances, laid out the same way, at a cost that follows the hits rather than the number of points."""
+        q = _to_matrix(points, self._dim) if not isinstance(points, np.ndarray) else points
+        return self._ix.graph_range_search(q, radius, ef_search=ef_search or 0)
 
     @staticmethod
     def _link_kw(config):

@@ -28,6 +28,7 @@ SYMBOLS = [
     "idb_last_search_full_fetches", "idb_debug_screen_bound", "idb_last_search_kernel", "idb_debug_merge_topk",
     "idb_exact_search_batch_f32", "idb_exact_search_batch_device_lane", "idb_index_insert_f32", "idb_index_load_storage",
     "idb_range_search_batch_f32", "idb_range_search_batch_device_lane", "idb_index_remove",
+    "idb_graph_range_search_batch_f32", "idb_graph_range_search_batch_device_lane",
 ]
 
 
@@ -87,6 +88,9 @@ def lib():
     L.idb_exact_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, vp, vp, vp]
     L.idb_range_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_float, C.c_uint64, u64p, u32p, f32p]
     L.idb_range_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_float, C.c_uint64, vp, vp, vp, u64p]
+    L.idb_graph_range_search_batch_f32.argtypes = [vp, f32p, C.c_uint64, C.c_uint32, C.c_float, C.c_uint64, u64p, u32p, f32p]
+    L.idb_graph_range_search_batch_device_lane.argtypes = [vp, C.c_uint32, vp, C.c_uint64, C.c_uint32, C.c_float, C.c_uint64, vp, vp, vp,
+                                                           u64p]
     L.idb_last_search_counters.argtypes = [vp, C.c_uint64, u64p]
     L.idb_last_search_failures.argtypes = [vp, C.c_uint32, u32p]
     L.idb_last_search_retried.argtypes = [vp, C.c_uint32, u32p]
@@ -167,6 +171,16 @@ def _storage(storage):
     if storage not in STORAGE:
         raise ValueError(f"storage must be one of {sorted(STORAGE)}, not {storage!r}")
     return STORAGE[storage]
+
+
+def _ef(ef_search):
+    """A search width as the C ABI's uint32_t: a value ctypes would wrap (negative, or 2^32 and up) is refused here."""
+    ef = int(ef_search)
+    if not 0 <= ef <= 0xFFFFFFFF:
+        raise ValueError(f"ef_search must be 0 (the index's) or 1..1024, not {ef_search!r}")
+    return ef
+
+
 PROGRESS_FN = C.CFUNCTYPE(None, C.c_uint64, C.c_uint64, C.c_void_p)
 
 
@@ -333,6 +347,19 @@ class Index:
         """Exact range search (idb_range_search_batch_f32): every point within `radius` of each query, as CSR (offsets u64 [nq + 1],
         ids u32 [total], dist f32 [total]); query i's hits are ids[offsets[i]:offsets[i + 1]], nearest first.  capacity=None: a first
         guess, and once more with the exact total when the hits did not fit."""
+        return self._csr(lambda q, nq, cap, o, i, d: lib().idb_range_search_batch_f32(self._h, q, nq, float(radius), cap, o, i, d),
+                         queries, capacity)
+
+    def graph_range_search(self, queries, radius, ef_search=0, capacity=None):
+        """Graph range search (idb_graph_range_search_batch_f32): the points within `radius` that layer 0 reaches from each query's
+        approximate nearest neighbours (ef_search: 0 = the index's) — a subset of range_search()'s result, laid out the same way."""
+        ef_search = _ef(ef_search)
+        return self._csr(lambda q, nq, cap, o, i, d: lib().idb_graph_range_search_batch_f32(self._h, q, nq, ef_search, float(radius),
+                                                                                            cap, o, i, d), queries, capacity)
+
+    def _csr(self, call, queries, capacity):
+        """A range entry call(queries, nq, capacity, offsets, ids, dist) as CSR; capacity=None: a first guess, and once more with the
+        exact total when the hits did not fit."""
         q = self._queries(queries)
         nq = q.shape[0]
         guess = capacity is None
@@ -341,9 +368,8 @@ class Index:
         while True:
             ids = np.empty(cap, dtype=np.uint32)
             dist = np.empty(cap, dtype=np.float32)
-            st = lib().idb_range_search_batch_f32(self._h, ptr(q, C.c_float), nq, float(radius), cap, ptr(offsets, C.c_uint64),
-                                                  ptr(ids, C.c_uint32), ptr(dist, C.c_float))
-            if st == ERR_CAPACITY and guess:
+            st = call(ptr(q, C.c_float), nq, cap, ptr(offsets, C.c_uint64), ptr(ids, C.c_uint32), ptr(dist, C.c_float))
+            if st == ERR_CAPACITY and guess and int(offsets[-1]) > cap:  # (a graph range search's seed overflow is not a size)
                 guess, cap = False, int(offsets[-1])
                 continue
             check(st)
@@ -356,6 +382,18 @@ class Index:
         total = C.c_uint64()
         st = lib().idb_range_search_batch_device_lane(self._h, lane, d_queries, nq, float(radius), capacity, d_offsets, d_ids, d_dist,
                                                        C.byref(total))
+        if st == ERR_CAPACITY:
+            raise IdbError(st, lib().idb_last_error().decode("utf-8", "replace") + f" (total {int(total.value)})")
+        check(st)
+        return int(total.value)
+
+    def graph_range_search_device(self, d_queries, nq, radius, capacity, d_offsets, d_ids, d_dist, ef_search=0, lane=0):
+        """Graph range search on device buffers on submission lane `lane`; returns the total (raises IdbError with status
+        ERR_CAPACITY, the offsets written, when it exceeds `capacity`).  Returns once the lane has run the call."""
+        ef_search = _ef(ef_search)
+        total = C.c_uint64()
+        st = lib().idb_graph_range_search_batch_device_lane(self._h, lane, d_queries, nq, ef_search, float(radius), capacity, d_offsets,
+                                                             d_ids, d_dist, C.byref(total))
         if st == ERR_CAPACITY:
             raise IdbError(st, lib().idb_last_error().decode("utf-8", "replace") + f" (total {int(total.value)})")
         check(st)

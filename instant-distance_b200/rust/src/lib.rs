@@ -42,6 +42,8 @@ extern "C" {
     fn idb_exact_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, k: u32, ids: *mut u32, dist: *mut f32, len: *mut u32) -> i32;
     fn idb_range_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32) -> i32;
     fn idb_range_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32, total: *mut u64) -> i32;
+    fn idb_graph_range_search_batch_f32(ix: *mut IdbIndex, q: *const f32, nq: u64, ef: u32, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32) -> i32;
+    fn idb_graph_range_search_batch_device_lane(ix: *mut IdbIndex, lane: u32, q: *const f32, nq: u64, ef: u32, radius: f32, capacity: u64, offsets: *mut u64, ids: *mut u32, dist: *mut f32, total: *mut u64) -> i32;
     fn idb_index_insert_f32(ix: *mut IdbIndex, rows: *const f32, m: u64, dim: u32, p: *const IdbParams, global_ids: *const u32, out_ids: *mut u32) -> i32;
     fn idb_index_remove(ix: *mut IdbIndex, pids: *const u32, m: u64, p: *const IdbParams, out_new_ids: *mut u32) -> i32;
     fn idb_index_free(ix: *mut IdbIndex);
@@ -195,6 +197,23 @@ impl Hnsw {
             let (mut ids, mut dist) = (vec![u32::MAX; cap], vec![f32::INFINITY; cap]);
             let rc = unsafe {
                 idb_range_search_batch_f32(self.raw, point.0.as_ptr(), 1, radius, cap as u64, offsets.as_mut_ptr(), ids.as_mut_ptr(), dist.as_mut_ptr())
+            };
+            if rc == 7 && offsets[1] as usize > cap { cap = offsets[1] as usize; continue; } // IDB_ERR_CAPACITY: once more, sized exactly
+            assert_eq!(rc, 0, "{}", last_error());
+            return (0..offsets[1] as usize).map(|i| (dist[i], PointId(ids[i]))).collect();
+        }
+    }
+    /// Not in the reference: the points within `radius` of `point` that layer 0 reaches from its `ef_search` approximate nearest
+    /// neighbours through points within `radius` (0: the index's ef_search), nearest first, ties by lower PointId, as (distance,
+    /// PointId).  A subset of search_range's result, at a cost that follows the hits rather than the number of points.
+    pub fn search_range_graph(&self, point: &F32Point, radius: f32, ef_search: u32) -> Vec<(f32, PointId)> {
+        let mut offsets = [0u64; 2];
+        let mut cap = 1024usize;
+        loop {
+            let (mut ids, mut dist) = (vec![u32::MAX; cap], vec![f32::INFINITY; cap]);
+            let rc = unsafe {
+                idb_graph_range_search_batch_f32(self.raw, point.0.as_ptr(), 1, ef_search, radius, cap as u64, offsets.as_mut_ptr(),
+                                                 ids.as_mut_ptr(), dist.as_mut_ptr())
             };
             if rc == 7 && offsets[1] as usize > cap { cap = offsets[1] as usize; continue; } // IDB_ERR_CAPACITY: once more, sized exactly
             assert_eq!(rc, 0, "{}", last_error());
