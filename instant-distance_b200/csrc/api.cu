@@ -3,7 +3,7 @@
 // Host side of the drop-in boundary: the index object, whose row-major point matrix (rows.cu) and per-layer fixed-stride adjacency
 // ("CSR with implicit row_ptr = pid * stride", rows INVALID-terminated; graph.cu) live in HBM, and the sm_90a kernels' launches.
 // No PyTorch, no CPU fallback: if the CUDA runtime reports no device every compute entry point fails loudly.
-#include "internal.cuh"
+#include "search_kernel.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -26,25 +26,12 @@ idb_status fail(idb_status st, const char* fmt, ...) {
     return st;
 }
 
-// one translation unit per CH (search_chN.cu)
-cudaError_t dispatch_search_ch1(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_ch2(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_ch3(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_ch4(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_ch6(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_ch8(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-cudaError_t dispatch_search_long(const SearchArgs&, int, int, int, cudaStream_t, const LaunchWindow&);
-
 static cudaError_t dispatch_search(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    switch (kernel_ch(a.g.nchunks)) {
-        case 1: return dispatch_search_ch1(a, row_t, ef_t, grid, st, win);
-        case 2: return dispatch_search_ch2(a, row_t, ef_t, grid, st, win);
-        case 3: return dispatch_search_ch3(a, row_t, ef_t, grid, st, win);
-        case 4: return dispatch_search_ch4(a, row_t, ef_t, grid, st, win);
-        case 6: return dispatch_search_ch6(a, row_t, ef_t, grid, st, win);
-        case 8: return dispatch_search_ch8(a, row_t, ef_t, grid, st, win);
-        default: return dispatch_search_long(a, row_t, ef_t, grid, st, win);
-    }
+    return with_cell(a.g.nchunks, [&](auto cell) {
+        constexpr int CH = decltype(cell)::CH;
+        if (a.g.row_type == kRowBin) return search_cells<CH, true>(a, row_t, ef_t, grid, st, win);
+        return search_cells<CH, false>(a, row_t, ef_t, grid, st, win);
+    });
 }
 
 __global__ void distance_kernel(const float4* a, const float4* b, uint32_t nchunks, float* out) {

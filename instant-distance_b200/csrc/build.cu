@@ -19,24 +19,12 @@
 
 namespace idb {
 
-cudaError_t build_dispatch_ch1(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_ch2(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_ch3(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_ch4(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_ch6(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_ch8(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-cudaError_t build_dispatch_long(const BuildArgs&, const BuildLaunch&, cudaStream_t);
-
 static cudaError_t build_dispatch_any(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    switch (kernel_ch(a.g.nchunks)) {
-        case 1: return build_dispatch_ch1(a, l, st);
-        case 2: return build_dispatch_ch2(a, l, st);
-        case 3: return build_dispatch_ch3(a, l, st);
-        case 4: return build_dispatch_ch4(a, l, st);
-        case 6: return build_dispatch_ch6(a, l, st);
-        case 8: return build_dispatch_ch8(a, l, st);
-        default: return build_dispatch_long(a, l, st);
-    }
+    return with_cell(a.g.nchunks, [&](auto cell) {
+        constexpr int CH = decltype(cell)::CH;
+        if (a.g.row_type == kRowBin) return build_cells<CH, true>(a, l, st);
+        return build_cells<CH, false>(a, l, st);
+    });
 }
 
 namespace {

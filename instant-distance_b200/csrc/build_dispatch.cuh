@@ -1,4 +1,4 @@
-// build_dispatch.cuh — launch helpers for the construction kernels, instantiated once per CH in build_chN.cu.
+// build_dispatch.cuh — launch helpers for the construction kernels, instantiated once per CH and row family in build_cells.cu.
 #pragma once
 #include "build_kernels.cuh"
 
@@ -32,8 +32,10 @@ cudaError_t launch_k2(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st)
     return cudaGetLastError();
 }
 
-template <int CH, int B, int NB, class RT>
+// The construction kernels of Cell<CH> for row type RT: B rows in flight per lane, as is, in KA and in K2 / K2'.
+template <int CH, class RT>
 cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
+    constexpr int B = Cell<CH>::B;
     switch (l.op) {
         case kOpInsertSearch:
             return with_tile(l.row_t, l.ef_t, [&](auto row, auto ef) {
@@ -43,9 +45,9 @@ cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStre
         case kOpSelectNew:
         case kOpRelink:
             if constexpr (CH > 0) {
-                if (l.stage) return launch_k2<CH, NB, true, RT>(a, l, st);
+                if (l.stage) return launch_k2<CH, B, true, RT>(a, l, st);
             }
-            return launch_k2<CH, NB, false, RT>(a, l, st);
+            return launch_k2<CH, B, false, RT>(a, l, st);
         case kOpRelinkSimple: {
             const int smem = CH == 0 ? (int)long_q_bytes(a.g.nchunks) * kBuildWarps : 0;
             auto kern = relink_simple_kernel<CH, RT>;
@@ -59,36 +61,9 @@ cudaError_t build_dispatch_rt(const BuildArgs& a, const BuildLaunch& l, cudaStre
     }
     return cudaErrorInvalidValue;
 }
-// The construction cells of bin rows (DESIGN §3d): declared here and defined in bin_cells.cuh, which only build_bin_chN.cu includes,
-// so that they compile in translation units of their own, in parallel with build_chN.cu's cells of the other row types.
-template <int CH, int B, int NB>
-cudaError_t build_dispatch_bin(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st);
-template <int CH, int B, int NB>
-cudaError_t build_dispatch(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st) {
-    return with_row_type(a.g.row_type, [&](auto rt) {
-        using RT = decltype(rt);
-        if constexpr (RT::kType == kRowBin) return build_dispatch_bin<CH, B, NB>(a, l, st);
-        else return build_dispatch_rt<CH, B, NB, RT>(a, l, st);
-    });
-}
-
-// K2's ladder, for other kernels built on select_heuristic_warp (remove.cu): f(CH, NB) as integral constants, with the (CH, NB) that
-// build_chN.cu instantiates for rows of `nchunks` chunks.
-template <int CH_, int NB_>
-struct K2Cell {
-    static constexpr int CH = CH_, NB = NB_;
-};
-template <class F>
-cudaError_t with_k2_cell(uint32_t nchunks, F&& f) {
-    switch (kernel_ch(nchunks)) {
-        case 1: return f(K2Cell<1, 16>());
-        case 2: return f(K2Cell<2, 8>());
-        case 3: return f(K2Cell<3, 4>());
-        case 4: return f(K2Cell<4, 4>());
-        case 6: return f(K2Cell<6, 2>());
-        case 8: return f(K2Cell<8, 2>());
-        default: return f(K2Cell<0, kLongRowsInFlight>());
-    }
-}
+// The construction cells of Cell<CH> for bin rows (BIN) or for f32, bf16, fp16 and q8 rows: defined in build_cells.cu, which is
+// compiled once per (CH, BIN) so that the cells build in parallel (DESIGN §3d).
+template <int CH, bool BIN>
+cudaError_t build_cells(const BuildArgs& a, const BuildLaunch& l, cudaStream_t st);
 
 }  // namespace idb

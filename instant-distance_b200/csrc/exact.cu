@@ -142,20 +142,11 @@ struct ScanChoice {
     ScanKernel fn;
     int qw;
 };
-template <int CH>
-ScanChoice scan_choice(uint32_t row_type) {
-    return with_row_type(row_type, [](auto rt) { return ScanChoice{exact_scan_kernel<CH, decltype(rt)>, ScanShape<CH>::QW}; });
-}
 ScanChoice pick_scan(uint32_t nchunks, uint32_t row_type) {
-    switch (kernel_ch(nchunks)) {
-        case 1: return scan_choice<1>(row_type);
-        case 2: return scan_choice<2>(row_type);
-        case 3: return scan_choice<3>(row_type);
-        case 4: return scan_choice<4>(row_type);
-        case 6: return scan_choice<6>(row_type);
-        case 8: return scan_choice<8>(row_type);
-        default: return scan_choice<0>(row_type);
-    }
+    return with_cell(nchunks, [&](auto cell) {
+        constexpr int CH = decltype(cell)::CH;
+        return with_row_type(row_type, [](auto rt) { return ScanChoice{exact_scan_kernel<CH, decltype(rt)>, ScanShape<CH>::QW}; });
+    });
 }
 
 }  // namespace

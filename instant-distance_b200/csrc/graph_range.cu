@@ -31,11 +31,10 @@ uint32_t pow2_at_least(uint64_t v) {
 }
 
 GraphRangeKernel pick_graph_range(const Index* ix) {
-    const int ch = kernel_ch(ix->nchunks);
     return with_row_type(ix->row_type, [&](auto rt) -> GraphRangeKernel {
         using RT = decltype(rt);
-        if constexpr (RT::kType == kRowBin) return graph_range_bin_cell(ch);
-        else return graph_range_cell<RT>(ch);
+        if constexpr (RT::kType == kRowBin) return graph_range_bin_cell(ix->nchunks);
+        else return graph_range_cell<RT>(ix->nchunks);
     });
 }
 

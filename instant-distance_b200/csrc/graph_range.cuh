@@ -149,22 +149,16 @@ __global__ void __launch_bounds__(kGrWarps * 32) graph_range_kernel(GraphRangeAr
 
 using GraphRangeKernel = void (*)(GraphRangeArgs);
 
-// The cell for rows of kernel_ch(nchunks) = CH chunks per lane and row type RT: K1's rows in flight per lane (search_chN.cu).
-template <int CH>
-constexpr int gr_rows_b() { return CH == 1 ? 16 : CH == 2 ? 8 : CH <= 4 ? 4 : 2; }
+// The cell for rows of nchunks chunks and row type RT: K1's rows in flight per lane, rows_in_flight<B, RT>() of with_cell's Cell (the
+// long rows, CH 0, take B as is).
 template <class RT>
-GraphRangeKernel graph_range_cell(int ch) {
-    switch (ch) {
-        case 1: return graph_range_kernel<1, rows_in_flight<gr_rows_b<1>(), RT>(), RT>;
-        case 2: return graph_range_kernel<2, rows_in_flight<gr_rows_b<2>(), RT>(), RT>;
-        case 3: return graph_range_kernel<3, rows_in_flight<gr_rows_b<3>(), RT>(), RT>;
-        case 4: return graph_range_kernel<4, rows_in_flight<gr_rows_b<4>(), RT>(), RT>;
-        case 6: return graph_range_kernel<6, rows_in_flight<gr_rows_b<6>(), RT>(), RT>;
-        case 8: return graph_range_kernel<8, rows_in_flight<gr_rows_b<8>(), RT>(), RT>;
-        default: return graph_range_kernel<0, kLongRowsInFlight, RT>;
-    }
+GraphRangeKernel graph_range_cell(uint32_t nchunks) {
+    return with_cell(nchunks, [](auto cell) -> GraphRangeKernel {
+        using C = decltype(cell);
+        return graph_range_kernel<C::CH, C::CH == 0 ? C::B : rows_in_flight<C::B, RT>(), RT>;
+    });
 }
 // graph_range_bin.cu
-GraphRangeKernel graph_range_bin_cell(int ch);
+GraphRangeKernel graph_range_bin_cell(uint32_t nchunks);
 
 }  // namespace idb

@@ -695,7 +695,7 @@ __device__ __forceinline__ bool vis_reserve(VisitedSet& v, uint32_t incoming, in
 // K1 phase clock (compile-time switch IDB_K1_PHASES, off in the product build; scripts/k1_phases.py builds a copy with it on).
 // search_layer adds clock64() deltas per warp to one tally per phase of an expansion; a phase ends where its loads have been
 // consumed, so a tally holds the phase's issue AND the wait for its own loads.  Each search_layer call of K1 adds its tallies to
-// g_k1_phases (one copy per translation unit: search_ch1.cu's is read by idb_debug_k1_phases).
+// g_k1_phases (one copy per translation unit: search_cells.cu's CH 1 f32 object's is read by idb_debug_k1_phases).
 // ---------------------------------------------------------------------------------------------------------
 #ifdef IDB_K1_PHASES
 enum K1Phase : int {

@@ -46,6 +46,27 @@ constexpr int kernel_ch(uint32_t nchunks) {
     return c <= 4 ? (int)c : c <= 6 ? 6 : c <= 8 ? 8 : 0;
 }
 
+// The traversal cell of CH = kernel_ch(nchunks): B is its rows in flight per lane for f32 rows.  K1 and the graph range expansion
+// take rows_in_flight<B, RT>() of it (search_kernel.cuh); KA, K2 / K2' and repair_kernel take B as is.
+template <int CH_>
+struct Cell {
+    static constexpr int CH = CH_;
+    static constexpr int B = CH == 1 ? 16 : CH == 2 ? 8 : CH == 3 || CH == 4 ? 4 : CH == 6 || CH == 8 ? 2 : kLongRowsInFlight;
+};
+// f(Cell<kernel_ch(nchunks)>()): the one switch from a row's chunk count to the cell compiled for it.
+template <class F>
+auto with_cell(uint32_t nchunks, F&& f) {
+    switch (kernel_ch(nchunks)) {
+        case 1: return f(Cell<1>());
+        case 2: return f(Cell<2>());
+        case 3: return f(Cell<3>());
+        case 4: return f(Cell<4>());
+        case 6: return f(Cell<6>());
+        case 8: return f(Cell<8>());
+        default: return f(Cell<0>());
+    }
+}
+
 // The big visited tier a traversal's warps bind (Index::select_visited_tier, DeviceCtx::retry_tier).
 struct VisTier {
     TablePool pool;                    // per-warp scratch tables, claimed per CTA (hnsw_device.cuh)

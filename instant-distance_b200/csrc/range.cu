@@ -113,20 +113,11 @@ struct RangeChoice {
     RangeKernel fn;
     int qw;
 };
-template <int CH>
-RangeChoice range_choice(uint32_t row_type) {
-    return with_row_type(row_type, [](auto rt) { return RangeChoice{range_scan_kernel<CH, decltype(rt)>, ScanShape<CH>::QW}; });
-}
 RangeChoice pick_range(uint32_t nchunks, uint32_t row_type) {
-    switch (kernel_ch(nchunks)) {
-        case 1: return range_choice<1>(row_type);
-        case 2: return range_choice<2>(row_type);
-        case 3: return range_choice<3>(row_type);
-        case 4: return range_choice<4>(row_type);
-        case 6: return range_choice<6>(row_type);
-        case 8: return range_choice<8>(row_type);
-        default: return range_choice<0>(row_type);
-    }
+    return with_cell(nchunks, [&](auto cell) {
+        constexpr int CH = decltype(cell)::CH;
+        return with_row_type(row_type, [](auto rt) { return RangeChoice{range_scan_kernel<CH, decltype(rt)>, ScanShape<CH>::QW}; });
+    });
 }
 
 unsigned grid_for(const Index* ix, uint64_t items) {

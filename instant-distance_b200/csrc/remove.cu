@@ -197,8 +197,8 @@ cudaError_t launch_repair(const RepairArgs& a, int grid, uint32_t smem_per_warp,
 }
 
 cudaError_t repair_dispatch(const RepairArgs& a, bool stage, int grid, uint32_t smem_per_warp, cudaStream_t st) {
-    return with_k2_cell(a.g.nchunks, [&](auto cell) {
-        constexpr int CH = decltype(cell)::CH, NB = decltype(cell)::NB;
+    return with_cell(a.g.nchunks, [&](auto cell) {
+        constexpr int CH = decltype(cell)::CH, NB = decltype(cell)::B;
         return with_row_type(a.g.row_type, [&](auto rt) {
             using RT = decltype(rt);
             if constexpr (CH > 0) {

@@ -222,8 +222,7 @@ extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* quer
     if (!index || (npairs && (!queries || !pairs || !out_bound || !out_dist))) return fail(IDB_ERR_INVALID_ARG, "null argument");
     Index* ix = reinterpret_cast<Index*>(index);
     if (!ix->d_codes) return fail(IDB_ERR_UNSUPPORTED, "this index has no screening table (IDB_SCREEN=0, empty, q8 or bin rows, or a non-finite value)");
-    const int ch = kernel_ch(ix->nchunks);
-    if (ch == 0) return fail(IDB_ERR_UNSUPPORTED, "dim %u: rows of more than 1024 elements are not screened", ix->dim);
+    if (kernel_ch(ix->nchunks) == 0) return fail(IDB_ERR_UNSUPPORTED, "dim %u: rows of more than 1024 elements are not screened", ix->dim);
     for (uint64_t i = 0; i < npairs; ++i)
         if (pairs[2 * i] >= nq || pairs[2 * i + 1] >= ix->n) return fail(IDB_ERR_INVALID_ARG, "pair %llu out of range", (unsigned long long)i);
     if (npairs == 0) return IDB_OK;
@@ -244,14 +243,11 @@ extern "C" idb_status idb_debug_screen_bound(idb_index* index, const float* quer
     if (e == cudaSuccess) {
         const GraphView g = ix->view();
         const float4* q4 = reinterpret_cast<const float4*>(dq);
-        switch (ch) {
-            case 1: e = launch_screen_bound<1>(g, q4, dp, npairs, dbound, ddist, st); break;
-            case 2: e = launch_screen_bound<2>(g, q4, dp, npairs, dbound, ddist, st); break;
-            case 3: e = launch_screen_bound<3>(g, q4, dp, npairs, dbound, ddist, st); break;
-            case 4: e = launch_screen_bound<4>(g, q4, dp, npairs, dbound, ddist, st); break;
-            case 6: e = launch_screen_bound<6>(g, q4, dp, npairs, dbound, ddist, st); break;
-            default: e = launch_screen_bound<8>(g, q4, dp, npairs, dbound, ddist, st); break;
-        }
+        e = with_cell(ix->nchunks, [&](auto cell) {
+            constexpr int CH = decltype(cell)::CH;
+            if constexpr (CH == 0) return cudaErrorInvalidValue;  // refused above
+            else return launch_screen_bound<CH>(g, q4, dp, npairs, dbound, ddist, st);
+        });
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_bound, dbound, ob, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, ddist, ob, cudaMemcpyDeviceToHost, st);

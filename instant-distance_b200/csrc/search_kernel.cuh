@@ -1,6 +1,6 @@
 // search_kernel.cuh — the traversal driver K1 and the build's KA share, K1: batched Hnsw::search kernel (lib.rs:352-383 per query),
 // and the traversal kernels' launch helpers.
-// Instantiated once per CH (float4 chunks per lane) in search_chN.cu so the translation units build in parallel.
+// Instantiated once per CH (float4 chunks per lane) and row family in search_cells.cu so the translation units build in parallel.
 #pragma once
 #include <cstring>
 #include <type_traits>
@@ -206,17 +206,9 @@ cudaError_t dispatch_row_ef_rt(const SearchArgs& a, int row_t, int ef_t, int gri
 // takes it too, one register per chunk as q8).
 template <int B, class RT>
 constexpr int rows_in_flight() { return RT::kChunkBytes <= 8 && 2 * B <= 16 ? 2 * B : B; }
-// K1's bin-row cells (DESIGN §3d): declared here and defined in bin_cells.cuh, which only search_bin_chN.cu includes, so that they
-// are compiled in translation units of their own, in parallel with search_chN.cu's cells of the other row types.
-template <int CH, int B>
-cudaError_t dispatch_row_ef_bin(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win);
-template <int CH, int B>
-cudaError_t dispatch_row_ef(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win) {
-    return with_row_type(a.g.row_type, [&](auto rt) {
-        using RT = decltype(rt);
-        if constexpr (RT::kType == kRowBin) return dispatch_row_ef_bin<CH, B>(a, row_t, ef_t, grid, st, win);
-        else return dispatch_row_ef_rt<CH, rows_in_flight<B, RT>(), RT>(a, row_t, ef_t, grid, st, win);
-    });
-}
+// K1's cells of Cell<CH> for bin rows (BIN) or for f32, bf16, fp16 and q8 rows: defined in search_cells.cu, which is compiled once
+// per (CH, BIN) so that the cells build in parallel (DESIGN §3d).
+template <int CH, bool BIN>
+cudaError_t search_cells(const SearchArgs& a, int row_t, int ef_t, int grid, cudaStream_t st, const LaunchWindow& win);
 
 }  // namespace idb

@@ -1,8 +1,8 @@
 """CPU statement of K1's dispatch: which instantiation of `search_kernel<CH, ROW_T, EF_T, B, OCC, RT, FULL, TMA>` a search launches.
 
-It restates, in plain Python, what `Index::enqueue_search` (api.cu), `dispatch_search`, `dispatch_search_ch1` (the IDB_VARIANT
-cases), `dispatch_row_ef`, `dispatch_row_ef_rt` and `launch_search_full` (search_kernel.cuh) decide, so that the GPU tests can check
-the cell `idb_last_search_kernel` reports against it and can prove that every compiled cell was run.
+It restates, in plain Python, what `Index::enqueue_search` and `dispatch_search` (api.cu), `with_cell` and `Cell` (internal.cuh),
+`search_cells` (search_cells.cu, with the IDB_VARIANT cases) and `dispatch_row_ef_rt` (search_kernel.cuh) decide, so that the GPU
+tests can check the cell `idb_last_search_kernel` reports against it and can prove that every compiled cell was run.
 
 A cell is (ch, row_t, ef_t, b, bf16, full, tma, variant): the fields of `Index.last_kernel()`.
 """
@@ -11,7 +11,7 @@ from collections import namedtuple
 Cell = namedtuple("Cell", "ch row_t ef_t b bf16 full tma variant")
 
 REGISTER_CH = (1, 2, 3, 4, 6, 8)  # float4 chunks per lane held in registers; 0 is the long-row kernel (query in shared memory)
-ROWS_IN_FLIGHT = {1: 16, 2: 8, 3: 4, 4: 4, 6: 2, 8: 2, 0: 8}  # B of f32 rows per CH (search_chN.cu)
+ROWS_IN_FLIGHT = {1: 16, 2: 8, 3: 4, 4: 4, 6: 2, 8: 2, 0: 8}  # B of f32 rows per CH (internal.cuh Cell)
 EF_TILES = {2: (4, 8, 16, 32), 4: (4, 16, 32)}  # EF_T instantiated per ROW_T: ROW_T 4 has no EF_T 8
 # IDB_VARIANT cases of the CH-1 headline shape (ROW_T 2, EF_T 4, f32 rows, never FULL): variant -> (B, TMA)
 VARIANTS = {1: (8, 0), 2: (8, 0), 3: (4, 0), 4: (16, 0), 5: (16, 1), 6: (8, 1), 7: (8, 1), 8: (32, 1)}

@@ -1,6 +1,6 @@
 """CPU statement of K1's dispatch for every row type, fp16 included: which instantiation of
 `search_kernel<CH, ROW_T, EF_T, B, OCC, RT, FULL, TMA>` a search launches (`Index::enqueue_search`, `dispatch_search`,
-`dispatch_search_ch1`, `dispatch_row_ef`, `dispatch_row_ef_rt`).
+`with_cell`, `search_cells`, `dispatch_row_ef_rt`).
 
 tests/k1_dispatch.py states the f32 and bf16 dispatch; this restates it with the row type as an IDB_STORAGE_* value, so that the
 fp16 GPU tests can check the cell `idb_last_search_kernel` reports, and tests/test_f16_cpu.py checks that it agrees with
